@@ -4,6 +4,7 @@ from __future__ import annotations
 import os
 import subprocess
 import sys
+import tempfile
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
@@ -89,13 +90,22 @@ def _build_f64(force=False, verbose=False):
 
 def build_variant(path, defines=(), force=False):
     """A build of the float32 engine with extra -D macros (test-only: e.g. MW_SMCON=6 makes almost every env take the
-    overflow path, whose results must be bit-identical to the standard build; tests/test_gpu.py)."""
+    overflow path, whose results must be bit-identical to the standard build; tests/test_gpu.py).  Returns the library's
+    path: `path`, or a file of the same name in a per-user temporary directory when `path`'s directory cannot be written
+    (tests may run from a read-only checkout)."""
     write_header()
+    try:
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        writable = os.access(os.path.dirname(path), os.W_OK)
+    except OSError:
+        writable = False
+    if not writable:
+        path = os.path.join(tempfile.gettempdir(), f"metaworld_b200-{os.getuid()}", os.path.basename(path))
+        os.makedirs(os.path.dirname(path), exist_ok=True)
     srcs = [os.path.join(CSRC, f) for f in SOURCES + HEADERS + ["mw_model.h", "mw_task_ids.h"]]
     if not force and os.path.exists(path) and os.path.getmtime(path) >= max(os.path.getmtime(d) for d in srcs):
         return path
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    os.makedirs(os.path.dirname(path), exist_ok=True)
     cmd = [nvcc] + [f"-D{d}" for d in defines] + NVCC_TARGET + ["-O3", "-lineinfo", "-std=c++17", "-DMW_NO_FASTMATH",
                                                   "-Xcompiler", "-fPIC", "-shared", "-o", path] + [os.path.join(CSRC, s) for s in SOURCES]
     r = subprocess.run(cmd, capture_output=True, text=True)

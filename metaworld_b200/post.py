@@ -14,222 +14,151 @@ episode-statistics wrapper (metaworld/__init__.py:437-444):
   running mean / variance (Welford merge of one-sample batches, initial count 1e-4) over every observation the wrapper
   sees, i.e. step observations AND reset observations; output float32.
 
-Pure numpy on [N, ...] arrays; `MetaWorldVecEnv` applies it to what the engine returns.  Because the reference puts
+Elementwise ops on [N, ...] arrays; `MetaWorldVecEnv` applies them to what the engine returns.  Because the reference puts
 `RecordEpisodeStatistics` outside the reward normalisation, the episodic return it reports is the sum of NORMALISED
-rewards; `ep_return` below tracks that."""
+rewards; `ep_return` below tracks that.
+
+The arithmetic is written once against a small array namespace: numpy for `step` / `reset`, torch for `step_torch` (on
+the device, without host synchronisation).  The per-env state lives in the namespace of the last call and is copied,
+exactly, when a call arrives in the other one.  The host path is not torch on CPU tensors because torch's CPU `sqrt` is
+not correctly rounded and numpy's is."""
 from __future__ import annotations
+
+from types import SimpleNamespace
 
 import numpy as np
 
+_NUMPY = SimpleNamespace(f32=np.dtype(np.float32), f64=np.dtype(np.float64), where=np.where, sqrt=np.sqrt, maybe_any=np.any,
+                         zeros=np.zeros, cast=lambda x, dtype: np.asarray(x, dtype=dtype),
+                         cat=lambda xs: np.concatenate(xs, axis=1), take=lambda x: x.cpu().numpy())
 
-class RunningMeanStdBatch:
-    """N independent copies of gymnasium's RunningMeanStd (wrappers/utils.py), each fed one sample per update: the
-    parallel-variance merge with batch mean = x, batch variance = 0, batch count = 1.  Arithmetic runs in `dtype`, with the
-    count converted at each use, like a Python-float count combined with float32 arrays in the per-env wrapper."""
 
-    def __init__(self, n, shape, dtype, epsilon=1e-4):
-        self.mean = np.zeros((n,) + tuple(shape), dtype=dtype)
-        self.var = np.ones((n,) + tuple(shape), dtype=dtype)
-        self.count = np.full(n, epsilon, dtype=np.float64)
-        self._bc = (n,) + (1,) * len(shape)
-
-    def update(self, x, mask=None):
-        dt = self.mean.dtype
-        count = self.count.reshape(self._bc)
-        tot = count + 1.0
-        c, tt = count.astype(dt), tot.astype(dt)
-        delta = np.asarray(x, dtype=dt) - self.mean
-        mean = self.mean + delta / tt
-        m2 = self.var * c + np.square(delta) * c / tt
-        var = m2 / tt
-        if mask is None:
-            self.mean, self.var, self.count = mean, var, self.count + 1.0
-        else:
-            m = np.asarray(mask, dtype=bool)
-            mb = m.reshape(self._bc)
-            self.mean, self.var = np.where(mb, mean, self.mean), np.where(mb, var, self.var)
-            self.count = np.where(m, self.count + 1.0, self.count)
+def _torch_namespace(device):
+    import torch
+    return SimpleNamespace(f32=torch.float32, f64=torch.float64, where=torch.where, sqrt=torch.sqrt,
+                           maybe_any=lambda x: True,    # finding out would synchronise with the device; the masked form is exact
+                           zeros=lambda shape, dtype: torch.zeros(shape, dtype=dtype, device=device),
+                           cast=lambda x, dtype: x.to(dtype), cat=lambda xs: torch.cat(xs, dim=1),
+                           take=lambda x: torch.from_numpy(x).to(device))
 
 
 class StepPost:
     GAMMA, EPS = 0.99, 1e-8          # gymnasium's defaults; the reference passes none
+    _STATE = ("mean", "var", "ret_mean", "ret_var", "ret_count", "disc", "obs_mean", "obs_var", "obs_count", "ep_return")
 
     def __init__(self, num_envs, recurrent_info_in_obs=False, normalize_reward_in_recurrent_info=True,
-                 reward_normalization_method=None, reward_alpha=0.001, normalize_observations=False):
+                 reward_normalization_method=None, reward_alpha=0.001, normalize_observations=False, obs_dtype=np.float64):
+        """`obs_dtype`: the dtype of the observations `on_step` gets on the host; the observation statistics are kept in it
+        (gymnasium's `RunningMeanStd(dtype=observation_space.dtype)`) whatever the dtype of a device observation."""
         if reward_normalization_method not in (None, "exponential", "gymnasium"):
             raise ValueError(f"unknown reward_normalization_method {reward_normalization_method!r}")
         self.n = num_envs
-        self.gym_reward = reward_normalization_method == "gymnasium"
-        self.norm_obs = bool(normalize_observations)
-        self.ret = RunningMeanStdBatch(num_envs, (), np.float64)      # NormalizeReward.return_rms of every sub-env
-        self.disc = np.zeros(num_envs)                                 # NormalizeReward.discounted_reward
-        self.obs_rms = None                                            # NormalizeObservation.obs_rms, shaped at the first observation
         self.recurrent = bool(recurrent_info_in_obs)
         self.norm_in_obs = bool(normalize_reward_in_recurrent_info)
         self.exponential = reward_normalization_method == "exponential"
+        self.gym_reward = reward_normalization_method == "gymnasium"
+        self.norm_obs = bool(normalize_observations)
         self.alpha = float(reward_alpha)
-        self.mean = np.zeros(num_envs)
-        self.var = np.ones(num_envs)
-        self.ep_return = np.zeros(num_envs)
         self.extra = 6 if self.recurrent else 0
+        self.obs_dtype = np.dtype(obs_dtype)
+        self.mean, self.var = np.zeros(num_envs), np.ones(num_envs)          # NormalizeRewardsExponential
+        # NormalizeReward.return_rms and .discounted_reward of every sub-env
+        self.ret_mean, self.ret_var, self.ret_count = np.zeros(num_envs), np.ones(num_envs), np.full(num_envs, 1e-4)
+        self.disc = np.zeros(num_envs)
+        self.obs_mean = self.obs_var = self.obs_count = None                # NormalizeObservation.obs_rms, shaped at the first call
+        self.ep_return = np.zeros(num_envs)
+        self.xp, self._torch = _NUMPY, None
 
     @property
     def active(self):
         return self.recurrent or self.exponential or self.gym_reward or self.norm_obs
 
-    def _normalize_obs(self, obs, mask=None):
-        """NormalizeObservation.observation on the rows selected by `mask` (all when None): update, then normalise."""
-        if self.obs_rms is None:
-            self.obs_rms = RunningMeanStdBatch(self.n, obs.shape[1:], obs.dtype)
-        self.obs_rms.update(obs, mask)
-        return np.float32((obs - self.obs_rms.mean) / np.sqrt(self.obs_rms.var + self.EPS))
-
-    def on_reset(self, obs, mask=None):
-        """obs [N, D] -> [N, D + extra]; the reward statistics are NOT reset (the wrapper object lives across episodes)."""
-        if mask is None:
-            self.ep_return[:] = 0
+    def _use(self, obs):
+        """The namespace of `obs`; the state is copied there when the previous call used the other one."""
+        if self.norm_obs and self.obs_mean is None:        # first call: the state is still in numpy
+            shape = (self.n, obs.shape[1] + self.extra)
+            self.obs_mean, self.obs_var = np.zeros(shape, self.obs_dtype), np.ones(shape, self.obs_dtype)
+            self.obs_count = np.full((self.n, 1), 1e-4)
+        if isinstance(obs, np.ndarray):
+            xp = _NUMPY
         else:
-            self.ep_return[mask] = 0
+            self._torch = self._torch or _torch_namespace(obs.device)
+            xp = self._torch
+        if xp is not self.xp:
+            for k in self._STATE:
+                if getattr(self, k) is not None:
+                    setattr(self, k, xp.take(getattr(self, k)))
+            self.xp = xp
+        return xp
+
+    @staticmethod
+    def _merge(xp, mean, var, count, x):
+        """N independent copies of gymnasium's RunningMeanStd.update (wrappers/utils.py), each fed one sample: the
+        parallel-variance merge with batch mean = x, batch variance = 0, batch count = 1.  Arithmetic runs in the dtype of
+        `mean`, with the float64 count converted at each use, like a Python-float count combined with float32 arrays in the
+        per-env wrapper.  -> (mean, var, count)"""
+        tot = count + 1.0
+        c, tt = xp.cast(count, mean.dtype), xp.cast(tot, mean.dtype)
+        delta = x - mean
+        return mean + delta / tt, (var * c + delta * delta * c / tt) / tt, tot
+
+    def _normalize_obs(self, xp, obs, mask=None):
+        """NormalizeObservation.observation on the rows selected by `mask` (all when None): update, then normalise."""
+        x = xp.cast(obs, self.obs_mean.dtype)
+        mean, var, count = self._merge(xp, self.obs_mean, self.obs_var, self.obs_count, x)
+        if mask is not None:
+            m = mask[:, None]
+            mean, var, count = xp.where(m, mean, self.obs_mean), xp.where(m, var, self.obs_var), xp.where(m, count, self.obs_count)
+        self.obs_mean, self.obs_var, self.obs_count = mean, var, count
+        return xp.cast((x - mean) / xp.sqrt(var + self.EPS), xp.f32)
+
+    def on_reset(self, obs):
+        """obs [N, D] -> [N, D + extra]; the reward statistics are NOT reset (the wrapper object lives across episodes)."""
+        xp = self._use(obs)
+        self.ep_return = xp.zeros(self.n, xp.f64)
         if self.recurrent:
-            obs = np.concatenate([obs, np.zeros((len(obs), 6), dtype=obs.dtype)], axis=1)
+            obs = xp.cat([obs, xp.zeros((self.n, 6), obs.dtype)])
         if self.norm_obs:
-            obs = self._normalize_obs(obs, mask)
+            obs = self._normalize_obs(xp, obs)
         return obs
 
-    def _update(self, r):
-        self.mean = (1 - self.alpha) * self.mean + self.alpha * r
-        self.var = (1 - self.alpha) * self.var + self.alpha * np.square(r - self.mean)
-
     def on_step(self, obs, actions, reward, terminated, truncated, final_obs=None):
-        """Returns (obs_out, reward_out, final_obs_out, episode_return_of_finished_envs).
-        `obs` holds the post-autoreset observation for finished envs (SAME_STEP) and `final_obs` their terminal one."""
-        done = np.logical_or(terminated, truncated)
+        """Returns (obs_out, reward_out [float64], final_obs_out, episode_return_of_finished_envs).
+        `obs` holds the post-autoreset observation for finished envs (SAME_STEP) and `final_obs` their terminal one; it
+        may be None when no env finished."""
+        xp = self._use(obs)
+        done = (terminated | truncated) != 0
+        reward = xp.cast(reward, xp.f64)
         obs_out, final_out = obs, final_obs
         if self.recurrent:
             r_obs = reward / 10.0 if self.norm_in_obs else reward
-            ext = np.concatenate([np.asarray(actions, dtype=obs.dtype).reshape(self.n, 4), r_obs[:, None].astype(obs.dtype),
-                                  done[:, None].astype(obs.dtype)], axis=1)
+            ext = xp.cat([xp.cast(actions, obs.dtype).reshape(self.n, 4), xp.cast(r_obs[:, None], obs.dtype),
+                          xp.cast(done[:, None], obs.dtype)])
             if final_obs is not None:
-                final_out = np.concatenate([final_obs, ext], axis=1)
-            ext = np.where(done[:, None], 0, ext).astype(obs.dtype)          # a freshly reset env reports zeros
-            obs_out = np.concatenate([obs, ext], axis=1)
+                final_out = xp.cat([final_obs, ext])
+            obs_out = xp.cat([obs, xp.where(done[:, None], 0, ext)])          # a freshly reset env reports zeros
         reward_out = reward
         if self.exponential:
-            self._update(reward)
-            self._update(reward)
-            reward_out = reward / (np.sqrt(self.var) + 1e-8)
+            for _ in range(2):          # the reference updates the estimate twice per step (wrappers.py:250-258)
+                self.mean = (1 - self.alpha) * self.mean + self.alpha * reward
+                d = reward - self.mean
+                self.var = (1 - self.alpha) * self.var + self.alpha * (d * d)
+            reward_out = reward / (xp.sqrt(self.var) + 1e-8)
         elif self.gym_reward:
-            self.disc = self.disc * self.GAMMA * (1 - terminated) + reward
-            self.ret.update(self.disc)
-            reward_out = reward / np.sqrt(self.ret.var + self.EPS)
+            self.disc = self.disc * self.GAMMA * (1.0 - xp.cast(terminated, xp.f64)) + reward
+            self.ret_mean, self.ret_var, self.ret_count = self._merge(xp, self.ret_mean, self.ret_var, self.ret_count, self.disc)
+            reward_out = reward / xp.sqrt(self.ret_var + self.EPS)
         if self.norm_obs:
             # the wrapper sees the step observation of every env (the terminal one for a finished env), then - SAME_STEP -
-            # the reset observation of the finished ones: two updates for those, in that order
-            if final_out is not None and done.any():
-                stepped = np.where(done[:, None], final_out, obs_out)
-                normed = self._normalize_obs(stepped)
+            # the reset observation of the finished ones: two updates for those, in that order.  The second one is masked,
+            # so it leaves the other envs' statistics as they were; the host skips it when no env finished
+            if final_out is not None and xp.maybe_any(done):
+                normed = self._normalize_obs(xp, xp.where(done[:, None], final_out, obs_out))
+                obs_out = xp.where(done[:, None], self._normalize_obs(xp, obs_out, done), normed)
                 final_out = normed
-                obs_out = np.where(done[:, None], self._normalize_obs(obs_out, done), normed)
             else:
-                obs_out = self._normalize_obs(obs_out)
-        self.ep_return += reward_out
-        finished = np.where(done, self.ep_return, 0.0)
-        self.ep_return[done] = 0
-        return obs_out, reward_out, final_out, finished
-
-
-class StepPostTorch:
-    """The same two wrappers on CUDA tensors, for `MetaWorldVecEnv.step_torch` (so RL code that keeps everything on the GPU
-    gets the recurrent observation and the normalised reward without a host round trip).  Plain torch elementwise ops on
-    [N, ...] tensors: plumbing around the engine's outputs, not a hot path."""
-
-    def __init__(self, torch, device, num_envs, obs_dim, recurrent_info_in_obs=False, normalize_reward_in_recurrent_info=True,
-                 reward_normalization_method=None, reward_alpha=0.001, normalize_observations=False):
-        self.t = torch
-        self.gym_reward = reward_normalization_method == "gymnasium"
-        self.norm_obs = bool(normalize_observations)
-        D = obs_dim + (6 if recurrent_info_in_obs else 0)
-        f64 = dict(device=device, dtype=torch.float64)
-        self.ret_mean, self.ret_var = torch.zeros(num_envs, **f64), torch.ones(num_envs, **f64)
-        self.ret_count = torch.full((num_envs,), 1e-4, **f64)
-        self.disc = torch.zeros(num_envs, **f64)
-        self.obs_mean, self.obs_var = torch.zeros(num_envs, D, **f64), torch.ones(num_envs, D, **f64)
-        self.obs_count = torch.full((num_envs, 1), 1e-4, **f64)
-        self.recurrent = bool(recurrent_info_in_obs)
-        self.norm_in_obs = bool(normalize_reward_in_recurrent_info)
-        self.exponential = reward_normalization_method == "exponential"
-        self.alpha = float(reward_alpha)
-        self.mean = torch.zeros(num_envs, device=device, dtype=torch.float64)
-        self.var = torch.ones(num_envs, device=device, dtype=torch.float64)
-        self.ep_return = torch.zeros(num_envs, device=device, dtype=torch.float64)
-        self.obs_dim = obs_dim
-        self.out = torch.zeros(num_envs, obs_dim + 6, device=device) if self.recurrent else None
-        self.final_out = torch.zeros(num_envs, obs_dim + 6, device=device) if self.recurrent else None
-
-    def load_host_state(self, post: StepPost):
-        """Continue from the numpy-path statistics (a run may mix `step` and `step_torch`)."""
-        t = self.t
-        self.mean.copy_(t.from_numpy(post.mean)); self.var.copy_(t.from_numpy(post.var)); self.ep_return.copy_(t.from_numpy(post.ep_return))
-        self.ret_mean.copy_(t.from_numpy(post.ret.mean)); self.ret_var.copy_(t.from_numpy(post.ret.var))
-        self.ret_count.copy_(t.from_numpy(post.ret.count)); self.disc.copy_(t.from_numpy(post.disc))
-        if post.obs_rms is not None:
-            self.obs_mean.copy_(t.from_numpy(post.obs_rms.mean.astype(np.float64))); self.obs_var.copy_(t.from_numpy(post.obs_rms.var.astype(np.float64)))
-            self.obs_count.copy_(t.from_numpy(post.obs_rms.count)[:, None])
-
-    @staticmethod
-    def _merge(mean, var, count, x):
-        """one-sample parallel-variance merge (RunningMeanStdBatch.update); count broadcasts over the trailing axes"""
-        tot = count + 1.0
-        delta = x - mean
-        return mean + delta / tot, (var * count + delta * delta * count / tot) / tot, tot
-
-    def _normalize_obs(self, obs, mask=None):
-        t = self.t
-        x = obs.double()
-        mean, var, count = self._merge(self.obs_mean, self.obs_var, self.obs_count, x)
-        if mask is None:
-            self.obs_mean, self.obs_var, self.obs_count = mean, var, count
-        else:
-            m = mask[:, None]
-            self.obs_mean, self.obs_var, self.obs_count = t.where(m, mean, self.obs_mean), t.where(m, var, self.obs_var), t.where(m, count, self.obs_count)
-        return ((x - self.obs_mean) / (self.obs_var + StepPost.EPS).sqrt()).float()
-
-    def on_reset(self, obs):
-        self.ep_return.zero_()
-        if self.recurrent:
-            self.out.zero_(); self.out[:, : self.obs_dim] = obs
-            obs = self.out
-        if self.norm_obs:
-            obs = self._normalize_obs(obs)
-        return obs
-
-    def on_step(self, obs, actions, reward, terminated, truncated, final_obs):
-        """-> (obs_out, reward_out [float64], final_obs_out, episode_return_of_finished_envs)"""
-        t = self.t
-        done = (terminated | truncated).bool()
-        r64 = reward.double()
-        obs_out, final_out = obs, final_obs
-        if self.recurrent:
-            r_obs = (r64 / 10.0 if self.norm_in_obs else r64).float()
-            ext = t.cat([actions, r_obs[:, None], done[:, None].float()], dim=1)
-            self.final_out[:, : self.obs_dim] = final_obs; self.final_out[:, self.obs_dim:] = ext
-            self.out[:, : self.obs_dim] = obs; self.out[:, self.obs_dim:] = t.where(done[:, None], t.zeros_like(ext), ext)
-            obs_out, final_out = self.out, self.final_out
-        reward_out = r64
-        if self.exponential:
-            for _ in range(2):          # the reference updates the estimate twice per step (wrappers.py:250-258)
-                self.mean = (1 - self.alpha) * self.mean + self.alpha * r64
-                self.var = (1 - self.alpha) * self.var + self.alpha * (r64 - self.mean) ** 2
-            reward_out = r64 / (self.var.sqrt() + 1e-8)
-        elif self.gym_reward:
-            self.disc = self.disc * StepPost.GAMMA * (1.0 - terminated.double()) + r64
-            self.ret_mean, self.ret_var, self.ret_count = self._merge(self.ret_mean, self.ret_var, self.ret_count, self.disc)
-            reward_out = r64 / (self.ret_var + StepPost.EPS).sqrt()
-        if self.norm_obs:       # every env's step observation first, then the reset observation of the finished ones (no sync: masked)
-            normed = self._normalize_obs(t.where(done[:, None], final_out, obs_out))
-            obs_out = t.where(done[:, None], self._normalize_obs(obs_out, done), normed)
-            final_out = normed
-        self.ep_return += reward_out
-        finished = t.where(done, self.ep_return, t.zeros_like(self.ep_return))
-        self.ep_return = t.where(done, t.zeros_like(self.ep_return), self.ep_return)
+                obs_out = self._normalize_obs(xp, obs_out)
+        self.ep_return = self.ep_return + reward_out
+        finished = xp.where(done, self.ep_return, 0.0)
+        self.ep_return = xp.where(done, 0.0, self.ep_return)
         return obs_out, reward_out, final_out, finished

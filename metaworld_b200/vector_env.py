@@ -200,16 +200,16 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self._closed = False
         self._needs_reset = True
         self._device_sampler = False
-        # optional per-sub-env wrappers of the reference that sit above the one-hot wrapper (metaworld/__init__.py:437-444)
+        # optional per-sub-env wrappers of the reference that sit above the one-hot wrapper (metaworld/__init__.py:437-444);
+        # one instance (one set of statistics) serves both `step` and `step_torch`
         from .post import StepPost
-        self.post = StepPost(N, recurrent_info_in_obs, normalize_reward_in_recurrent_info, reward_normalization_method, reward_alpha,
-                             normalize_observations)
-        if self.post.recurrent:     # RNNBasedMetaRLWrapper's space: unbounded float32 of obs + action + reward + done (wrappers.py:55-62)
-            D = self.obs_dim + self.post.extra
+        if recurrent_info_in_obs:
             self.obs_dtype = np.float32
-            self.single_observation_space = _gym.Box(np.full(D, -np.inf, np.float32), np.full(D, np.inf, np.float32), dtype=np.float32)
-            self.observation_space = _gym.batch_space(self.single_observation_space, num_envs)
-        if self.post.norm_obs:      # gymnasium.wrappers.NormalizeObservation: unbounded float32 space of the same shape
+        self.post = StepPost(N, recurrent_info_in_obs, normalize_reward_in_recurrent_info, reward_normalization_method, reward_alpha,
+                             normalize_observations, obs_dtype=self.obs_dtype)
+        if self.post.recurrent or self.post.norm_obs:
+            # RNNBasedMetaRLWrapper (obs + action + reward + done, wrappers.py:55-62) and gymnasium.wrappers.NormalizeObservation
+            # both declare an unbounded float32 space
             D = self.obs_dim + self.post.extra
             self.single_observation_space = _gym.Box(np.full(D, -np.inf, np.float32), np.full(D, np.inf, np.float32), dtype=np.float32)
             self.observation_space = _gym.batch_space(self.single_observation_space, num_envs)
@@ -400,7 +400,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         return self.step(self._pending_actions)
 
     # GPU-resident variants (no host synchronisation; task re-sampling on autoreset happens on the device).  The optional
-    # recurrent-obs / reward-normalisation wrappers are applied on the device as well (post.StepPostTorch).
+    # recurrent-obs / normalisation wrappers are applied on the device as well, by the same `post.StepPost` as `step`.
     def enable_device_sampler(self):
         """Autoreset draws the next goal on the device: uniform over the env's own task list, a counter-based hash of
         (seed, env, episode) -- the distribution of RandomTaskSelectWrapper, not its PCG64 stream.  The host task mirrors
@@ -417,18 +417,12 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self._device_sampler = False
         self._needs_reset = True
 
-    def _post_torch(self):
-        if getattr(self, "_ptorch", None) is None:
-            from .post import StepPostTorch
-            p = self.post
-            self._ptorch = StepPostTorch(self.torch, self.device, self.num_envs, self.obs_dim, p.recurrent, p.norm_in_obs,
-                                         "exponential" if p.exponential else "gymnasium" if p.gym_reward else None, p.alpha, p.norm_obs)
-            self._ptorch.load_host_state(p)
-        return self._ptorch
-
     def reset_torch(self):
-        self.reset()
-        return self._post_torch().on_reset(self.d_obs) if self.post.active else self.d_obs
+        obs, _ = self.reset()
+        if not self.post.active:
+            return self.d_obs
+        # the wrapped observation of reset(): the wrappers' statistics see the reset observation once
+        return self.torch.from_numpy(np.asarray(obs, dtype=np.float32)).to(self.device)
 
     def step_torch(self, actions):
         """`actions`: float32 CUDA tensor [num_envs, 4] on this env's device.  Returns device tensors (obs [N, obs_dim],
@@ -444,8 +438,8 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         nxt = None if self._device_sampler else self.d_next
         self.engine.step(actions, self.d_obs, self.d_reward, self.d_term, self.d_trunc, self.d_small, self.d_final_obs,
                          self.d_final_info, nxt)
-        if self.post.active:       # RNNBasedMetaRLWrapper / NormalizeRewardsExponential on the device; the terminal observation
-            obs, rew, self.d_final_obs_post, self.d_episode_return_post = self._post_torch().on_step(    # and episode returns stay available
+        if self.post.active:       # the optional wrappers on the device; the terminal observation and episode returns stay available
+            obs, rew, self.d_final_obs_post, self.d_episode_return_post = self.post.on_step(
                 self.d_obs, actions, self.d_reward, self.d_term, self.d_trunc, self.d_final_obs)
             return obs, rew, self.d_term, self.d_trunc, self.d_info
         return self.d_obs, self.d_reward, self.d_term, self.d_trunc, self.d_info

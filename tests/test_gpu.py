@@ -683,10 +683,19 @@ def test_fault_flags_are_clean_and_catch_nonfinite(torch_cuda):
 
 
 def test_step_torch_applies_recurrent_obs_and_reward_normalisation_on_device(torch_cuda):
-    """Row f1: the RNN-obs and exponential-reward wrappers on the GPU-resident path equal the numpy path."""
-    torch = torch_cuda
+    """Row f1: the RNN-obs and exponential-reward wrappers on the GPU-resident path equal the numpy path bit for bit
+    (torch's CUDA division and sqrt are correctly rounded, like numpy's)."""
+    _step_torch_equals_step(torch_cuda, dict(recurrent_info_in_obs=True, reward_normalization_method="exponential", reward_alpha=0.1))
+
+
+def test_step_torch_applies_observation_and_gymnasium_reward_normalisation_on_device(torch_cuda):
+    """Row f1: the same for gymnasium's NormalizeObservation (float32 statistics: one-hot observations) and NormalizeReward."""
+    _step_torch_equals_step(torch_cuda, dict(normalize_observations=True, reward_normalization_method="gymnasium"))
+
+
+def _step_torch_equals_step(torch, wrappers):
     from metaworld_b200.vector_env import make_mt_envs
-    kw = dict(seed=3, num_envs=10, max_episode_steps=6, use_one_hot=True, recurrent_info_in_obs=True, reward_normalization_method="exponential", reward_alpha=0.1)
+    kw = dict(seed=3, num_envs=10, max_episode_steps=6, use_one_hot=True, **wrappers)
     a, b = make_mt_envs("MT10", **kw), make_mt_envs("MT10", **kw)
     o1, _ = a.reset(); o2 = b.reset_torch()
     assert np.array_equal(o1, o2.cpu().numpy())
@@ -698,7 +707,7 @@ def test_step_torch_applies_recurrent_obs_and_reward_normalisation_on_device(tor
         act = rng.uniform(-1, 1, size=(10, 4)).astype(np.float32)
         x = a.step(act)
         y = b.step_torch(torch.tensor(act, device=b.device))
-        assert np.allclose(x[0], y[0].cpu().numpy(), atol=1e-6) and np.allclose(x[1], y[1].cpu().numpy(), atol=1e-9)
+        assert np.array_equal(x[0], y[0].cpu().numpy()) and np.array_equal(x[1], y[1].cpu().numpy())
         assert np.array_equal(x[2], y[2].cpu().numpy().astype(bool)) and np.array_equal(x[3], y[3].cpu().numpy().astype(bool))
     a.close(); b.close()
 

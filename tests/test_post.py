@@ -1,6 +1,7 @@
 """metaworld_b200.post.StepPost against scalar transcriptions of the reference wrappers it vectorises
 (metaworld/wrappers.py:35-88 RNNBasedMetaRLWrapper, :233-258 NormalizeRewardsExponential; stacking order and
-RecordEpisodeStatistics placement from metaworld/__init__.py:437-446)."""
+RecordEpisodeStatistics placement from metaworld/__init__.py:437-446), and against its recorded outputs
+(tests/golden/post_steppost.npz) on numpy and on torch inputs."""
 import numpy as np
 import pytest
 
@@ -62,27 +63,37 @@ def test_steppost_matches_scalar_wrappers():
                     assert np.allclose(o[i], so) and fin[i] == 0.0
 
 
-@pytest.mark.parametrize("cfg", [(True, True, "exponential", 0.05, False), (False, True, "gymnasium", 0.001, True),
-                                 (True, False, "gymnasium", 0.001, True), (False, True, None, 0.001, True)])
-def test_torch_variant_equals_numpy_variant(cfg):
-    """post.StepPostTorch (what step_torch applies on the device) against post.StepPost, on CPU tensors."""
+def _goldens():
+    """tests/golden/post_steppost.npz and the generator that wrote it (its configurations and input replay)"""
+    import importlib.util
+    import os
+    here = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+    spec = importlib.util.spec_from_file_location("make_post_goldens", os.path.join(here, "make_post_goldens.py"))
+    gen = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(gen)
+    z = np.load(os.path.join(here, "post_steppost.npz"))
+    return gen, z, {k[3:]: z[k] for k in z.files if k.startswith("in/")}
+
+
+GEN, GOLD, INPUTS = _goldens()
+
+
+@pytest.mark.parametrize("cfg", GEN.CONFIGS, ids=[GEN.config_name(*c) for c in GEN.CONFIGS])
+def test_numpy_inputs_match_goldens(cfg):
+    """The host path (`step` / `reset`) is bit-identical to the outputs recorded for every option combination."""
+    out = GEN.run(GEN.make_post(*cfg), INPUTS, cfg[-1])
+    for k, v in out.items():
+        g = GOLD[f"{GEN.config_name(*cfg)}/{k}"]
+        assert v.dtype == g.dtype and np.array_equal(v, g), k
+
+
+@pytest.mark.parametrize("cfg", GEN.CONFIGS, ids=[GEN.config_name(*c) for c in GEN.CONFIGS])
+def test_torch_inputs_match_goldens(cfg):
+    """The same arithmetic on CPU tensors (what `step_torch` runs on the device): only torch's CPU `sqrt`, which is not
+    correctly rounded, separates it from the goldens."""
     import torch
-    from metaworld_b200.post import StepPost, StepPostTorch
-    n, d = 6, 9
-    rng = np.random.default_rng(3)
-    a = StepPost(n, *cfg)
-    b = StepPostTorch(torch, torch.device("cpu"), n, d, *cfg)
-    o0 = rng.normal(size=(n, d)).astype(np.float32)
-    # (float32 statistics on the numpy side when the input is float32 - the recurrent wrapper's dtype -, float64 on the torch side)
-    assert np.allclose(a.on_reset(o0), b.on_reset(torch.from_numpy(o0)).numpy(), atol=1e-6, rtol=1e-3)
-    for t in range(12):
-        obs = rng.normal(size=(n, d)).astype(np.float32); fo = rng.normal(size=(n, d)).astype(np.float32)
-        act = rng.uniform(-1, 1, size=(n, 4)).astype(np.float32); rew = rng.uniform(0, 10, size=n)
-        term = rng.random(n) < 0.1; trunc = (t % 5 == 4) & ~term
-        x = a.on_step(obs, act, rew, term, trunc, final_obs=fo)
-        y = b.on_step(torch.from_numpy(obs), torch.from_numpy(act), torch.from_numpy(rew.astype(np.float32)), torch.from_numpy(term), torch.from_numpy(trunc), torch.from_numpy(fo))
-        r32 = rew.astype(np.float32).astype(np.float64)       # the device path sees the float32 reward
-        done = term | trunc
-        assert np.allclose(x[0], y[0].numpy(), atol=2e-5, rtol=1e-3)
-        assert np.allclose(x[2][done], y[2].numpy()[done], atol=2e-5, rtol=1e-3)          # terminal rows are defined for finished envs only
-        assert np.allclose(x[1], y[1].numpy(), rtol=1e-5) and np.allclose(x[3], y[3].numpy(), rtol=1e-5, atol=1e-6)
+    post = GEN.make_post(*cfg)
+    out = GEN.run(post, INPUTS, cfg[-1], convert=torch.from_numpy, back=lambda t: t.numpy())
+    assert isinstance(post.ep_return, torch.Tensor)           # the state moved to torch and stayed there
+    for k, v in out.items():
+        np.testing.assert_allclose(v, GOLD[f"{GEN.config_name(*cfg)}/{k}"], rtol=1e-6, atol=0, err_msg=k)

@@ -134,6 +134,40 @@ def test_pseudorandom_task_cycle_and_attribute_rpc():
         env.get_attr("no_such_attribute")
 
 
+def test_optional_wrappers_keep_one_state_across_numpy_and_torch_paths():
+    """The optional wrappers' statistics are shared by `step` and `step_torch`: reset_torch() returns the uploaded output of
+    reset(), so the observation statistics count the reset observation once, and a run that alternates the two step paths
+    follows the all-numpy run up to torch's CPU `sqrt` rounding."""
+    kw = dict(max_episode_steps=3, task_select="pseudorandom", use_one_hot=True, num_tasks=2, recurrent_info_in_obs=True,
+              reward_normalization_method="gymnasium", normalize_observations=True)
+    a, _ = make(["reach-v3", "push-v3"], 4, **kw)
+    b, _ = make(["reach-v3", "push-v3"], 4, **kw)
+    oa, _ = a.reset()
+    ob = b.reset_torch()
+    assert np.array_equal(oa, ob.numpy()) and np.array_equal(np.asarray(b.post.obs_count), np.full((4, 1), 1 + 1e-4))
+    rng = np.random.default_rng(0)
+    n_done = 0
+    for t in range(10):
+        act = rng.uniform(-1, 1, size=(4, 4)).astype(np.float32)
+        obs, rew, term, trunc, info = a.step(act)
+        done = term | trunc
+        if t % 2:
+            o2, r2, term2, trunc2, info2 = b.step(act)
+            fo2 = np.stack([info2["final_obs"][e] for e in np.nonzero(done)[0]]) if done.any() else None
+            ep2 = info2["final_info"]["episode"]["r"] if done.any() else None
+        else:
+            o2, r2, term2, trunc2, _ = (x.numpy() for x in b.step_torch(torch.from_numpy(act)))
+            fo2, ep2 = b.d_final_obs_post.numpy()[done], np.asarray(b.d_episode_return_post)
+        assert np.array_equal(term, term2 != 0) and np.array_equal(trunc, trunc2 != 0)
+        np.testing.assert_allclose(o2, obs, rtol=1e-6, atol=0)
+        np.testing.assert_allclose(r2, rew, rtol=1e-6, atol=0)
+        if done.any():
+            n_done += int(done.sum())
+            np.testing.assert_allclose(fo2, np.stack([info["final_obs"][e] for e in np.nonzero(done)[0]]), rtol=1e-6, atol=0)
+            np.testing.assert_allclose(ep2, info["final_info"]["episode"]["r"], rtol=1e-6, atol=0)
+    assert n_done >= 8
+
+
 def test_checkpoint_round_trip_restores_task_stream():
     """Reference format (metaworld/wrappers.py:125-142,275-322): (env_id, dict) per sub-env; a second env that loads it
     continues with the same task sequence (cross-checked against the reference itself in tests/test_refpin_vector.py)."""
