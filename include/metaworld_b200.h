@@ -62,19 +62,39 @@ int mw_get_snapshots(mw_engine*, int first, int n, void* out);
 int mw_reset(mw_engine*, int n, const int* env_ids /*DEV or NULL*/, const int* snapshot_ids /*DEV*/,
              float* obs /*DEV*/, int obs_stride, void* stream);
 
-/* VectorEnv.step with SAME_STEP autoreset (metaworld/__init__.py:465,491-509 ->
- * SawyerXYZEnv.step, metaworld/sawyer_xyz_env.py:580-642 + TimeLimit + AutoTerminateOnSuccessWrapper,
- * metaworld/wrappers.py:207-230).  All arrays DEV, n_envs rows:
+/* VectorEnv.step (metaworld/__init__.py:465,491-509 -> SawyerXYZEnv.step, metaworld/sawyer_xyz_env.py:580-642 +
+ * TimeLimit + AutoTerminateOnSuccessWrapper, metaworld/wrappers.py:207-230), autoreset as set by mw_set_autoreset_mode
+ * (default SAME_STEP).  All arrays DEV, n_envs rows:
  *   actions [n,4] f32; obs [n,obs_stride] f32 (39 written); reward [n] f32; terminated/truncated [n] u8;
  *   info [n,info_stride] f32, columns 0..6 = success, near_object, grasp_success, grasp_reward, in_place_reward,
  *   obj_to_target, unscaled_reward; when info_stride >= 9 also column 7 = reward and column 8 = terminated + 2*truncated
- *   (one packed record per env for a single device->host copy); final_obs [n,obs_stride] / final_info [n,8] (7 infos + episode return) are written
- *   only for rows whose episode ended in this call (terminated|truncated), which then restart from
- *   next_snapshot[i] (or, when next_snapshot is NULL, from a snapshot drawn on the device from the env's
- *   own goal set, see mw_set_goal_sets).                                                             */
+ *   (one packed record per env for a single device->host copy).
+ * SAME_STEP: final_obs [n,obs_stride] / final_info [n,8] (7 infos + episode return) are written only for rows whose
+ *   episode ended in this call (terminated|truncated), which then restart from next_snapshot[i] (or, when next_snapshot
+ *   is NULL, from a snapshot drawn on the device from the env's own goal set, see mw_set_goal_sets).
+ * NEXT_STEP: an ending episode reports its terminal observation in obs and its return in final_info column 7 (nothing
+ *   else of final_obs / final_info is written); the env is marked as ended.  The next call restarts it as SAME_STEP
+ *   would have (same snapshot choice) and reports the reset observation, reward 0, no flags, an all-zero info row
+ *   (columns 7 and 8 included); its action is ignored.
+ * DISABLED: an ending episode reports its terminal observation and its return (final_info column 7), and the env is
+ *   marked as ended.  Stepping an ended env
+ *   leaves its state and output rows untouched and sets MW_FAULT_STEP_AFTER_END (restart it with mw_reset_masked).
+ * An ended env's warp still runs the physics of the step (its CTA's warps meet at every phase barrier) and discards it:
+ *   mw_get_counters counts that pass in env steps [1] and forward passes [4], not in contacts dropped [2] or solver
+ *   iterations [3]; it reports no fault other than MW_FAULT_STEP_AFTER_END.                                          */
 int mw_step(mw_engine*, const float* actions, float* obs, int obs_stride, float* reward,
             unsigned char* terminated, unsigned char* truncated, float* info, int info_stride, float* final_obs,
             float* final_info, const int* next_snapshot, void* stream);
+
+/* gymnasium.vector.AutoresetMode of mw_step; other values fail with MW_ERR_ARG.  Takes effect at the next launch. */
+enum mw_autoreset_mode { MW_AUTORESET_SAME_STEP = 0, MW_AUTORESET_NEXT_STEP = 1, MW_AUTORESET_DISABLED = 2 };
+int mw_set_autoreset_mode(mw_engine*, int mode);
+
+/* VectorEnv.reset(options={"reset_mask": mask}): every env with mask[i] != 0 restarts from snapshot_ids[i] (NULL: a
+ * snapshot drawn by the device sampler, as in mw_step) and clears its ended mark; its episode counter advances by one, as
+ * in an autoreset (mw_reset sets it to 0).  obs row i (not compacted) is written for those envs only.  mask DEV u8 [n_envs],
+ * snapshot_ids DEV [n_envs] or NULL, obs DEV float [n_envs, obs_stride].                                             */
+int mw_reset_masked(mw_engine*, const unsigned char* mask, const int* snapshot_ids, float* obs, int obs_stride, void* stream);
 
 /* SawyerXYZEnv.evaluate_state(obs, action) (metaworld/sawyer_xyz_env.py:644-656 -> the task's evaluate_state /
  * compute_reward): reward and info of every env's CURRENT physics state for caller-supplied observations and actions.
@@ -87,7 +107,9 @@ int mw_evaluate(mw_engine*, const float* actions, const float* obs, int obs_stri
  *   1 MW_FAULT_TOL_BOUNDS  reward_utils.tolerance: lower > upper          (ValueError, reward_utils.py:124-125)
  *   2 MW_FAULT_TOL_MARGIN  reward_utils.tolerance: margin < 0             (ValueError, reward_utils.py:134-135)
  *   4 MW_FAULT_HAMACHER    hamacher_product input outside [0, 1]          (ValueError, reward_utils.py:237-238)
- *   8 MW_FAULT_NONFINITE   non-finite observation or reward (the reference's `_did_see_sim_exception` path)      */
+ *   8 MW_FAULT_NONFINITE   non-finite observation or reward (the reference's `_did_see_sim_exception` path)
+ *  16 MW_FAULT_STEP_AFTER_END  DISABLED autoreset: stepped after its episode ended, before mw_reset_masked (gymnasium's
+ *                              SyncVectorEnv asserts; SawyerXYZEnv.step raises past max_path_length).  API misuse.   */
 int mw_get_faults(mw_engine*, int* out);
 
 /* options: max_episode_steps (TimeLimit), terminate_on_success (0/1), device sampler seed */

@@ -34,7 +34,7 @@ def entry_points():
 
     def mt(name):
         def vec(seed=None, use_one_hot=False, num_envs=None, vector_strategy="sync", autoreset_mode=None, **kw):
-            return V.make_mt_envs(name, seed=seed, use_one_hot=use_one_hot, num_envs=num_envs, **kw)
+            return V.make_mt_envs(name, seed=seed, use_one_hot=use_one_hot, num_envs=num_envs, autoreset_mode=autoreset_mode, **kw)
         return vec
 
     def ml(name, split):
@@ -42,14 +42,14 @@ def entry_points():
             # make_ml_envs_train / _test partials (metaworld/__init__.py:596-604)
             kw.setdefault("terminate_on_success", split == "test")
             return V.make_ml_envs(kw.pop("env_name", name), seed=seed, meta_batch_size=meta_batch_size, total_tasks_per_cls=total_tasks_per_cls,
-                                  split=split, num_envs=num_envs, **kw)
+                                  split=split, num_envs=num_envs, autoreset_mode=autoreset_mode, **kw)
         return vec
 
     def mt1_single(env_name, use_one_hot=False, seed=None, num_envs=None, vector_strategy="sync", autoreset_mode=None, **kw):
         return V.make_mt_envs(env_name, seed=seed, use_one_hot=use_one_hot, single=True, **kw)      # gym.make -> ONE wrapped env
 
     def mt1_vec(env_name, use_one_hot=False, seed=None, num_envs=None, vector_strategy="sync", autoreset_mode=None, **kw):
-        return V.make_mt_envs(env_name, seed=seed, use_one_hot=use_one_hot, num_envs=num_envs, **kw)
+        return V.make_mt_envs(env_name, seed=seed, use_one_hot=use_one_hot, num_envs=num_envs, autoreset_mode=autoreset_mode, **kw)
 
     table = {"MT1": (mt1_single, mt1_vec)}
     for n in ("MT10", "MT25", "MT50"):
@@ -60,11 +60,12 @@ def entry_points():
     table["goal_hidden"] = (lambda env_name, seed=None, **kw: S.make_goal_env(env_name, seed, observable=False, **kw), None)
     table["goal_observable"] = (lambda env_name, seed=None, **kw: S.make_goal_env(env_name, seed, observable=True, **kw), None)
     table["custom-mt-envs"] = (None, lambda envs_list, seed=None, use_one_hot=False, num_envs=None, vector_strategy="sync", autoreset_mode=None, **kw:
-                               V.make_custom_mt_envs(envs_list, seed=seed, use_one_hot=use_one_hot, num_envs=num_envs, **kw))
+                               V.make_custom_mt_envs(envs_list, seed=seed, use_one_hot=use_one_hot, num_envs=num_envs, autoreset_mode=autoreset_mode, **kw))
     table["custom-ml-envs"] = (None, lambda train_envs, test_envs, seed=None, meta_batch_size=20, total_tasks_per_cls=None, num_envs=None,
                                vector_strategy="sync", autoreset_mode=None, **kw:
                                V.make_custom_ml_envs(train_envs, test_envs, seed=seed, meta_batch_size=meta_batch_size,
-                                                     total_tasks_per_cls=total_tasks_per_cls, num_envs=num_envs, **kw))
+                                                     total_tasks_per_cls=total_tasks_per_cls, num_envs=num_envs, autoreset_mode=autoreset_mode,
+                                                     **kw))
     return table
 
 

@@ -1,7 +1,7 @@
 // libmwb200: batched Meta-World step engine for H100 (sm_90a).  C ABI: include/metaworld_b200.h.
 //
 // One warp = one environment for a whole env step: 5 x (forward dynamics + semi-implicit Euler), one more
-// forward pass, observation, reward/info, time-limit / success termination and SAME_STEP autoreset, with the
+// forward pass, observation, reward/info, time-limit / success termination and autoreset (SAME_STEP, NEXT_STEP or none), with the
 // per-env state making a single 512-byte round trip to HBM (coalesced 128-bit loads/stores).  One CTA = WARPS_PER_BLOCK warps
 // that share one task model; the ~10 KB model blob is staged into shared memory with a TMA bulk copy
 // (cp.async.bulk + mbarrier).  There is no CPU fallback: every entry point launches CUDA kernels or fails.
@@ -45,6 +45,7 @@ struct EngineDev {
   unsigned* env_cycles;                              // [n_envs] cycles each env's warp spent in its previous k_step = duration of its CTA (orders the CTAs, k_order_blocks)
   unsigned* env_prof;                                // optional [n_envs][16] per-env phase cycles / event counts of the last step (mw_set_profiling)
   int n_envs, max_steps, terminate_on_success; unsigned long long seed;
+  int autoreset_mode;                                // MW_AUTORESET_* (mw_set_autoreset_mode)
 };
 
 // The per-warp global scratch (EPA polytope, overflow rows) is addressed by SM, not by CTA, when at most one CTA fits an SM:
@@ -147,8 +148,16 @@ DEV void make_obs(const TaskCtx& c, float* obs, bool clip = true) {   // reset()
 DEV unsigned long long mix64(unsigned long long x) {
   x += 0x9E3779B97F4A7C15ull; x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull; x = (x ^ (x >> 27)) * 0x94D049BB133111EBull; return x ^ (x >> 31);
 }
+// device task sampler: the snapshot env `env` restarts from after its episode number `episode` (mw_set_goal_sets)
+DEV int sample_snapshot(const EngineDev& e, int env, float episode) {
+  unsigned long long h = mix64(e.seed ^ mix64(((unsigned long long)env << 32) | (unsigned)(int)episode));
+  return e.goal_first[env] + (int)(h % (unsigned long long)e.goal_count[env]);
+}
 
 // ---------------------------------------------------------------- kernels
+// DEFERRED = false: SAME_STEP autoreset; true: NEXT_STEP or DISABLED (e.autoreset_mode tells which).  Two instantiations,
+// so that the default path carries none of the code of the other modes (the kernel is bound by instruction fetch)
+template <bool DEFERRED>
 __global__ void __launch_bounds__(BLOCK_THREADS, 1)
 k_step(EngineDev e, const int* __restrict__ block_order, const int* __restrict__ block_model, const int* __restrict__ block_start, const int* __restrict__ block_count,
        const int* __restrict__ perm, const float* __restrict__ actions, float* __restrict__ obs_out, int obs_stride,
@@ -172,6 +181,9 @@ k_step(EngineDev e, const int* __restrict__ block_order, const int* __restrict__
   join_cta(bs, wsa, w, warp, block_count[blk]);
   const MwModel* m = (const MwModel*)bs->model;
   load_env(ws, e.state + env, lane);
+  // NEXT_STEP / DISABLED: an env whose episode ended in the previous call still runs its physics below, so that its warp
+  // takes part in the CTA's phase barriers, and the result is discarded in the tail (restart, or nothing at all)
+  const bool ended = DEFERRED && ws->es.ended != 0.f;
   if (lane < 16) w->prof[lane] = 0;
   if (lane == 0) { w->fault = 0; w->prof_on = e.prof != nullptr; }
   SYNCW();
@@ -212,11 +224,13 @@ k_step(EngineDev e, const int* __restrict__ block_order, const int* __restrict__
     ws->es.ep_return += (float)rew;
     bool trunc = ws->es.path_len >= (float)e.max_steps;
     bool term = e.terminate_on_success && inf[INFO_SUCCESS] == (real)1;
-    reward[env] = (float)rew; terminated[env] = term; truncated[env] = trunc;
-    if (info_stride >= 9) { info_out[(size_t)env * info_stride + 7] = (float)rew; info_out[(size_t)env * info_stride + 8] = (float)((int)term + 2 * (int)trunc); }   // packed record: one D2H copy
     ws->info[7] = (term || trunc) ? 1.f : 0.f;
-    { bool fin = isfinite((float)rew); for (int i = 0; i < 39; i++) fin = fin && isfinite(ws->obs[i]); if (!fin) w->fault |= MW_FAULT_NONFINITE; }
-    e.diag[3 * env] += dropped; e.diag[3 * env + 1] += iters; e.diag[3 * env + 2] |= w->fault;
+    if (!ended) {
+      reward[env] = (float)rew; terminated[env] = term; truncated[env] = trunc;
+      if (info_stride >= 9) { info_out[(size_t)env * info_stride + 7] = (float)rew; info_out[(size_t)env * info_stride + 8] = (float)((int)term + 2 * (int)trunc); }   // packed record: one D2H copy
+      { bool fin = isfinite((float)rew); for (int i = 0; i < 39; i++) fin = fin && isfinite(ws->obs[i]); if (!fin) w->fault |= MW_FAULT_NONFINITE; }
+      e.diag[3 * env] += dropped; e.diag[3 * env + 1] += iters; e.diag[3 * env + 2] |= w->fault;
+    } else if (e.autoreset_mode == MW_AUTORESET_DISABLED) e.diag[3 * env + 2] |= MW_FAULT_STEP_AFTER_END;   // the discarded pass reports nothing else
     w->prof[7] = MW_CLK(w) - t_phys; w->prof[8] = MW_CLK(w) - t_begin;
     // launch-order key: the cycles this env spent in its constraint solver + constraint assembly.  The whole-step time
     // is the same for all warps of a CTA (they wait for each other at every phase boundary) and would keep light envs
@@ -242,20 +256,35 @@ k_step(EngineDev e, const int* __restrict__ block_order, const int* __restrict__
     }
   }
   done = ws->info[7] != 0.f;
-  if (lane < INFO_N) info_out[(size_t)env * info_stride + lane] = ws->info[lane];
-  if (!done) {
-    for (int i = lane; i < 39; i += 32) obs_out[(size_t)env * obs_stride + i] = ws->obs[i];
-    store_env(ws, e.state + env, lane);
+  if (ended) {
+    if (e.autoreset_mode == MW_AUTORESET_DISABLED) return;      // state record and output rows stay as they are
+    // NEXT_STEP, the call after the terminal step: the action is ignored, the env restarts and reports the reset
+    // observation with reward 0, no done flags and an all-zero info row
+    if (lane < INFO_N) info_out[(size_t)env * info_stride + lane] = 0.f;
+    if (lane == 0) {
+      reward[env] = 0.f; terminated[env] = 0; truncated[env] = 0;
+      if (info_stride >= 9) { info_out[(size_t)env * info_stride + 7] = 0.f; info_out[(size_t)env * info_stride + 8] = 0.f; }
+    }
   } else {
+    if (lane < INFO_N) info_out[(size_t)env * info_stride + lane] = ws->info[lane];
+    if (!done || DEFERRED) {
+      // NEXT_STEP / DISABLED terminal step: the terminal observation goes to obs, the env is marked and restarts later;
+      // the episode return still goes to final_info column 7 (episode statistics)
+      if (DEFERRED && done) {
+        if (final_info && lane == 7) final_info[(size_t)env * 8 + 7] = ws->es.ep_return;
+        if (lane == 0) ws->es.ended = 1.f;
+      }
+      for (int i = lane; i < 39; i += 32) obs_out[(size_t)env * obs_stride + i] = ws->obs[i];
+      store_env(ws, e.state + env, lane);
+      return;
+    }
     // SAME_STEP autoreset: report the terminal transition, restart from a cached episode-start snapshot
     if (final_obs) for (int i = lane; i < 39; i += 32) final_obs[(size_t)env * obs_stride + i] = ws->obs[i];
     if (final_info) { if (lane < INFO_N) final_info[(size_t)env * 8 + lane] = ws->info[lane]; if (lane == 7) final_info[(size_t)env * 8 + 7] = ws->es.ep_return; }
-    int snap;
-    if (next_snapshot) snap = next_snapshot[env];
-    else {
-      unsigned long long h = mix64(e.seed ^ mix64(((unsigned long long)env << 32) | (unsigned)(int)ws->es.episode));
-      snap = e.goal_first[env] + (int)(h % (unsigned long long)e.goal_count[env]);
-    }
+  }
+  {
+    // restart (same snapshot choice and episode count in both modes, so NEXT_STEP runs the goal sequence of SAME_STEP)
+    const int snap = next_snapshot ? next_snapshot[env] : sample_snapshot(e, env, ws->es.episode);
     float episode = ws->es.episode + 1.f;
     const MwSnapshot* sp = e.snaps + snap;
     float4 v = ((const float4*)&sp->st)[lane];
@@ -340,6 +369,23 @@ __global__ void k_reset(EngineDev e, int n, const int* __restrict__ env_ids, con
   ((float4*)(e.state + env))[lane] = v;
   if (lane == 0) e.state[env].snapshot = (float)snapshot_ids[gw];
   for (int i = lane; i < 39; i += 32) obs[(size_t)gw * obs_stride + i] = sp->obs[i];
+}
+
+// partial reset, one warp per env: envs with mask[env] set restart from snapshot_ids[env] (NULL: the device sampler's draw)
+// and count one more episode, as the autoreset does; obs row env is written, the other rows are left alone
+__global__ void k_reset_masked(EngineDev e, const unsigned char* __restrict__ mask, const int* __restrict__ snapshot_ids,
+                               float* __restrict__ obs, int obs_stride) {
+  const int env = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (env >= e.n_envs || !mask[env]) return;
+  const float episode = e.state[env].episode;
+  const int snap = snapshot_ids ? snapshot_ids[env] : sample_snapshot(e, env, episode);
+  const MwSnapshot* sp = e.snaps + snap;
+  float4 v = ((const float4*)&sp->st)[lane];
+  __syncwarp();                                        // every lane has read `episode` before the record is overwritten
+  ((float4*)(e.state + env))[lane] = v;
+  __syncwarp();
+  if (lane == 0) { e.state[env].episode = episode + 1.f; e.state[env].snapshot = (float)snap; }
+  for (int i = lane; i < 39; i += 32) obs[(size_t)env * obs_stride + i] = sp->obs[i];
 }
 
 __global__ void __launch_bounds__(BLOCK_THREADS, 1)
@@ -530,12 +576,12 @@ struct mw_engine {
   // head split (k_order_blocks): the alternative CTAs follow the n_blocks regular ones in the block table
   int n_blocks_total = 0, n_split = 0, split_warps = 4, n_sm = 0; float split_frac = 0.f;
   int *d_split_head = nullptr, *d_split_alt = nullptr, *d_split_state = nullptr, *d_block_live = nullptr;
-  int max_steps = 500, terminate_on_success = 0; unsigned long long seed = 0;
+  int max_steps = 500, terminate_on_success = 0; unsigned long long seed = 0; int autoreset_mode = MW_AUTORESET_SAME_STEP;
   unsigned long long launches = 0, env_steps = 0;
   EngineDev dev() const {
     EngineDev e; e.models = d_models; e.model_stride = model_stride; e.taskconsts = d_tc; e.meshverts = d_meshptrs;
     e.state = d_state; e.snaps = d_snaps; e.goal_first = d_goal_first; e.goal_count = d_goal_count; e.diag = d_diag; e.epa = d_epa; e.spill = d_spill; e.slot_by_sm = slot_by_sm; e.prof = profiling ? d_prof : nullptr; e.model_cycles = d_model_cycles; e.env_cost = d_env_cost; e.env_cycles = order_by_cycles ? d_env_cycles : nullptr; e.env_prof = profiling ? d_env_prof : nullptr;
-    e.n_envs = n_envs; e.max_steps = max_steps; e.terminate_on_success = terminate_on_success; e.seed = seed; return e;
+    e.n_envs = n_envs; e.max_steps = max_steps; e.terminate_on_success = terminate_on_success; e.seed = seed; e.autoreset_mode = autoreset_mode; return e;
   }
 };
 
@@ -677,7 +723,8 @@ int mw_create(mw_engine** out, int device, int n_models, const void* models, con
   CK(cudaMemset(E->d_prof, 0, sizeof(unsigned long long) * 16));
   CK(cudaFuncSetAttribute(k_order_envs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(unsigned long long) * MW_SORT_MAX)));
   CK(cudaFuncSetAttribute(k_order_blocks, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(unsigned long long) * MW_SORT_MAX)));
-  CK(cudaFuncSetAttribute(k_step, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
+  CK(cudaFuncSetAttribute(k_step<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
+  CK(cudaFuncSetAttribute(k_step<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_snapshot, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_substeps, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_evaluate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
@@ -789,6 +836,24 @@ int mw_reset(mw_engine* E, int n, const int* env_ids, const int* snapshot_ids, f
   return MW_OK;
 }
 
+int mw_reset_masked(mw_engine* E, const unsigned char* mask, const int* snapshot_ids, float* obs, int obs_stride, void* stream) {
+  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_reset_masked: mw_set_envs not called");
+  if (!mask || !obs || obs_stride < 39) return fail(MW_ERR_ARG, "mw_reset_masked: bad arguments");
+  if (!snapshot_ids && !E->d_goal_first) return fail(MW_ERR_STATE, "mw_reset_masked: no snapshot_ids and no goal sets for the device sampler");
+  CK(cudaSetDevice(E->device));
+  k_reset_masked<<<(E->n_envs * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(E->dev(), mask, snapshot_ids, obs, obs_stride);
+  CK(cudaGetLastError());
+  E->launches++;
+  return MW_OK;
+}
+
+int mw_set_autoreset_mode(mw_engine* E, int mode) {
+  if (!E || (mode != MW_AUTORESET_SAME_STEP && mode != MW_AUTORESET_NEXT_STEP && mode != MW_AUTORESET_DISABLED))
+    return fail(MW_ERR_ARG, "mw_set_autoreset_mode: mode must be MW_AUTORESET_SAME_STEP, _NEXT_STEP or _DISABLED");
+  E->autoreset_mode = mode;
+  return MW_OK;
+}
+
 int mw_step(mw_engine* E, const float* actions, float* obs, int obs_stride, float* reward, unsigned char* terminated, unsigned char* truncated,
             float* info, int info_stride, float* final_obs, float* final_info, const int* next_snapshot, void* stream) {
   if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_step: mw_set_envs not called");
@@ -803,7 +868,8 @@ int mw_step(mw_engine* E, const float* actions, float* obs, int obs_stride, floa
     k_order_blocks<<<1, 1024, sizeof(unsigned long long) * Pb, (cudaStream_t)stream>>>(nb, E->d_block_start, E->d_block_count, E->d_perm, E->d_env_cost, E->order_by_cycles ? E->d_env_cycles : nullptr, E->d_block_order,
         E->n_blocks, E->n_split, E->d_split_head, E->d_split_alt, E->d_split_state, E->n_split ? E->d_block_live : nullptr, E->split_frac, E->n_sm);
   }
-  k_step<<<E->n_split ? E->n_blocks_total : E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_order, E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm,
+  auto* kern = E->autoreset_mode == MW_AUTORESET_SAME_STEP ? k_step<false> : k_step<true>;
+  kern<<<E->n_split ? E->n_blocks_total : E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_order, E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm,
       actions, obs, obs_stride, reward, terminated, truncated, info, info_stride, final_obs, final_info, next_snapshot, E->n_split ? E->d_block_live : nullptr);
   CK(cudaGetLastError());
   E->launches += 3; E->env_steps += (unsigned long long)E->n_envs;

@@ -24,7 +24,9 @@ struct MwEnvState {
   float partially_observable;
   float snapshot;            // snapshot slot this episode started from
   float episode;             // episodes completed (drives the device-side task sampler)
-  float ep_return, pad[4];
+  float ep_return;
+  float ended;               // 1: the last step ended the episode and the env has not restarted (NEXT_STEP / DISABLED autoreset)
+  float pad[3];
 };
 static_assert(sizeof(MwEnvState) == 128 * 4, "MwEnvState must be 128 floats");
 
@@ -48,6 +50,7 @@ enum { INFO_SUCCESS = 0, INFO_NEAR_OBJECT, INFO_GRASP_SUCCESS, INFO_GRASP_REWARD
 #define MW_FAULT_TOL_MARGIN 2
 #define MW_FAULT_HAMACHER 4
 #define MW_FAULT_NONFINITE 8
+#define MW_FAULT_STEP_AFTER_END 16   // DISABLED autoreset: an env was stepped after its episode ended (API misuse, not a GPU fault)
 DEV real tol_long_tail_f(int* fault, real x, real lo, real hi, real margin) {
   if (lo > hi) *fault |= MW_FAULT_TOL_BOUNDS;
   if (margin < 0) *fault |= MW_FAULT_TOL_MARGIN;

@@ -27,7 +27,7 @@ ENVSTATE_DTYPE = np.dtype([("qpos", "f8", 18), ("qvel", "f4", 17), ("warm", "f4"
                            ("prev_obs", "f4", 18), ("shift", "f4", 3), ("target", "f4", 3), ("obj_init", "f4", 3),
                            ("init_tcp", "f4", 3), ("scal", "f4", 16), ("path_len", "f4"),
                            ("partially_observable", "f4"), ("snapshot", "f4"), ("episode", "f4"), ("ep_return", "f4"),
-                           ("pad", "f4", 4)])
+                           ("ended", "f4"), ("pad", "f4", 3)])
 SNAPSHOT_DTYPE = np.dtype([("st", ENVSTATE_DTYPE), ("obs", "f4", 39), ("pad", "f4", 25)])
 INFO_KEYS = ["success", "near_object", "grasp_success", "grasp_reward", "in_place_reward", "obj_to_target",
              "unscaled_reward"]
@@ -54,6 +54,8 @@ def _load(path):
     L.mw_get_snapshots.argtypes = [vp, ip, ip, vp]
     L.mw_reset.argtypes = [vp, ip, vp, vp, vp, ip, vp]
     L.mw_step.argtypes = [vp, vp, vp, ip, vp, vp, vp, vp, ip, vp, vp, vp, vp]
+    L.mw_set_autoreset_mode.argtypes = [vp, ip]
+    L.mw_reset_masked.argtypes = [vp, vp, vp, vp, ip, vp]
     L.mw_set_options.argtypes = [vp, ip, ip, C.c_ulonglong]
     L.mw_set_goal_sets.argtypes = [vp, vp, vp]
     L.mw_get_state.argtypes = [vp, vp]
@@ -238,6 +240,17 @@ class Engine:
                           self._p(truncated), self._p(info), info.stride(0), self._p(final_obs), self._p(final_info),
                           self._p(next_snapshot), self._stream()))
 
+    AUTORESET_MODES = {"SameStep": 0, "NextStep": 1, "Disabled": 2}     # gymnasium.vector.AutoresetMode values -> MW_AUTORESET_*
+
+    def set_autoreset_mode(self, mode):
+        """`mode`: "SameStep" | "NextStep" | "Disabled" (mw_set_autoreset_mode); applies from the next `step`."""
+        _ck(lib().mw_set_autoreset_mode(self.h, self.AUTORESET_MODES.get(mode, -1)))
+
+    def reset_masked(self, mask, obs, snapshot_ids=None):
+        """Restarts the envs with `mask` set (uint8/bool device tensor [n_envs]) from `snapshot_ids` (int32 device tensor
+        [n_envs], read at the masked rows) or, when None, from the device sampler's draw; writes those rows of `obs`."""
+        _ck(lib().mw_reset_masked(self.h, self._p(mask), self._p(snapshot_ids), self._p(obs), obs.stride(0), self._stream()))
+
     def evaluate(self, actions, obs, out):
         """evaluate_state for every env's current state: out [n, 8] = info[7], reward (mw_evaluate)."""
         _ck(lib().mw_evaluate(self.h, self._p(actions), self._p(obs), obs.stride(0), self._p(out), self._stream()))
@@ -245,7 +258,9 @@ class Engine:
     FAULTS = {1: "tolerance: lower bound > upper bound (the reference raises ValueError, reward_utils.py:124)",
               2: "tolerance: margin < 0 (the reference raises ValueError, reward_utils.py:134)",
               4: "hamacher_product: input outside [0, 1] (the reference raises ValueError, reward_utils.py:237)",
-              8: "non-finite observation or reward"}
+              8: "non-finite observation or reward",
+              16: "stepped after its episode ended with autoreset disabled (reset it with reset_mask first; the reference's "
+                  "SawyerXYZEnv.step raises ValueError past max_path_length)"}
 
     def faults(self):
         """Per-env MW_FAULT_* bits since the last call (cleared)."""

@@ -40,7 +40,8 @@ def _get_task_names(envs) -> list[str]:
 def evaluation(agent: Agent, eval_envs, num_episodes: int = 50):
     """evaluation.py:48-105: run until every task has `num_episodes` finished episodes; successes are counted on the first
     `num_episodes` episodes of each task (in order of completion, env index breaking ties within a step), returns are the
-    first `num_episodes` episodic returns per task."""
+    first `num_episodes` episodic returns per task.  Like the reference, it reads `final_info`, so `eval_envs` must use the
+    default SAME_STEP autoreset."""
     terminate_on_success = bool(np.all(eval_envs.get_attr("terminate_on_success")))
     eval_envs.call("toggle_terminate_on_success", True)
     obs, _ = eval_envs.reset()

@@ -47,9 +47,12 @@ class StepPost:
     _STATE = ("mean", "var", "ret_mean", "ret_var", "ret_count", "disc", "obs_mean", "obs_var", "obs_count", "ep_return")
 
     def __init__(self, num_envs, recurrent_info_in_obs=False, normalize_reward_in_recurrent_info=True,
-                 reward_normalization_method=None, reward_alpha=0.001, normalize_observations=False, obs_dtype=np.float64):
+                 reward_normalization_method=None, reward_alpha=0.001, normalize_observations=False, obs_dtype=np.float64,
+                 same_step=True):
         """`obs_dtype`: the dtype of the observations `on_step` gets on the host; the observation statistics are kept in it
-        (gymnasium's `RunningMeanStd(dtype=observation_space.dtype)`) whatever the dtype of a device observation."""
+        (gymnasium's `RunningMeanStd(dtype=observation_space.dtype)`) whatever the dtype of a device observation.
+        `same_step`: the autoreset mode is SAME_STEP (a finished env's `obs` row is its reset observation); otherwise
+        (NEXT_STEP / DISABLED) it is the terminal one, and a restart is a row of `on_step(restart=...)` or `on_reset(mask=...)`."""
         if reward_normalization_method not in (None, "exponential", "gymnasium"):
             raise ValueError(f"unknown reward_normalization_method {reward_normalization_method!r}")
         self.n = num_envs
@@ -61,6 +64,7 @@ class StepPost:
         self.alpha = float(reward_alpha)
         self.extra = 6 if self.recurrent else 0
         self.obs_dtype = np.dtype(obs_dtype)
+        self.same_step = bool(same_step)
         self.mean, self.var = np.zeros(num_envs), np.ones(num_envs)          # NormalizeRewardsExponential
         # NormalizeReward.return_rms and .discounted_reward of every sub-env
         self.ret_mean, self.ret_var, self.ret_count = np.zeros(num_envs), np.ones(num_envs), np.full(num_envs, 1e-4)
@@ -112,47 +116,59 @@ class StepPost:
         self.obs_mean, self.obs_var, self.obs_count = mean, var, count
         return xp.cast((x - mean) / xp.sqrt(var + self.EPS), xp.f32)
 
-    def on_reset(self, obs):
-        """obs [N, D] -> [N, D + extra]; the reward statistics are NOT reset (the wrapper object lives across episodes)."""
+    def on_reset(self, obs, mask=None):
+        """obs [N, D] -> [N, D + extra]; the reward statistics are NOT reset (the wrapper object lives across episodes).
+        `mask` [N] bool: a partial reset (`reset_mask`); only those rows' state changes, and only those output rows mean
+        anything."""
         xp = self._use(obs)
-        self.ep_return = xp.zeros(self.n, xp.f64)
+        self.ep_return = xp.zeros(self.n, xp.f64) if mask is None else xp.where(mask, 0.0, self.ep_return)
         if self.recurrent:
             obs = xp.cat([obs, xp.zeros((self.n, 6), obs.dtype)])
         if self.norm_obs:
-            obs = self._normalize_obs(xp, obs)
+            obs = self._normalize_obs(xp, obs, mask)
         return obs
 
-    def on_step(self, obs, actions, reward, terminated, truncated, final_obs=None):
+    def on_step(self, obs, actions, reward, terminated, truncated, final_obs=None, restart=None):
         """Returns (obs_out, reward_out [float64], final_obs_out, episode_return_of_finished_envs).
-        `obs` holds the post-autoreset observation for finished envs (SAME_STEP) and `final_obs` their terminal one; it
-        may be None when no env finished."""
+        SAME_STEP: `obs` holds the post-autoreset observation for finished envs and `final_obs` their terminal one; it
+        may be None when no env finished.  NEXT_STEP: `restart` [N] bool marks the envs this call restarted (their `obs` row
+        is the reset observation, reward 0): they get the reset treatment - zero recurrent extension, observation statistics
+        updated with the reset observation, reward statistics untouched, reward 0 - and the others the step treatment."""
         xp = self._use(obs)
         done = (terminated | truncated) != 0
         reward = xp.cast(reward, xp.f64)
         obs_out, final_out = obs, final_obs
+        fresh = done if self.same_step else restart        # rows of `obs` that are reset observations (None: none)
         if self.recurrent:
             r_obs = reward / 10.0 if self.norm_in_obs else reward
             ext = xp.cat([xp.cast(actions, obs.dtype).reshape(self.n, 4), xp.cast(r_obs[:, None], obs.dtype),
                           xp.cast(done[:, None], obs.dtype)])
             if final_obs is not None:
                 final_out = xp.cat([final_obs, ext])
-            obs_out = xp.cat([obs, xp.where(done[:, None], 0, ext)])          # a freshly reset env reports zeros
+            obs_out = xp.cat([obs, ext if fresh is None else xp.where(fresh[:, None], 0, ext)])   # a freshly reset env reports zeros
         reward_out = reward
+        keep = (lambda new, old: new) if restart is None else (lambda new, old: xp.where(restart, old, new))
         if self.exponential:
+            mean, var = self.mean, self.var
             for _ in range(2):          # the reference updates the estimate twice per step (wrappers.py:250-258)
-                self.mean = (1 - self.alpha) * self.mean + self.alpha * reward
-                d = reward - self.mean
-                self.var = (1 - self.alpha) * self.var + self.alpha * (d * d)
+                mean = (1 - self.alpha) * mean + self.alpha * reward
+                d = reward - mean
+                var = (1 - self.alpha) * var + self.alpha * (d * d)
+            self.mean, self.var = keep(mean, self.mean), keep(var, self.var)
             reward_out = reward / (xp.sqrt(self.var) + 1e-8)
         elif self.gym_reward:
-            self.disc = self.disc * self.GAMMA * (1.0 - xp.cast(terminated, xp.f64)) + reward
-            self.ret_mean, self.ret_var, self.ret_count = self._merge(xp, self.ret_mean, self.ret_var, self.ret_count, self.disc)
+            disc = self.disc * self.GAMMA * (1.0 - xp.cast(terminated, xp.f64)) + reward
+            ret_mean, ret_var, ret_count = self._merge(xp, self.ret_mean, self.ret_var, self.ret_count, disc)
+            self.disc, self.ret_mean = keep(disc, self.disc), keep(ret_mean, self.ret_mean)
+            self.ret_var, self.ret_count = keep(ret_var, self.ret_var), keep(ret_count, self.ret_count)
             reward_out = reward / xp.sqrt(self.ret_var + self.EPS)
+        if restart is not None:
+            reward_out = xp.where(restart, 0.0, reward_out)
         if self.norm_obs:
             # the wrapper sees the step observation of every env (the terminal one for a finished env), then - SAME_STEP -
             # the reset observation of the finished ones: two updates for those, in that order.  The second one is masked,
             # so it leaves the other envs' statistics as they were; the host skips it when no env finished
-            if final_out is not None and xp.maybe_any(done):
+            if self.same_step and final_out is not None and xp.maybe_any(done):
                 normed = self._normalize_obs(xp, xp.where(done[:, None], final_out, obs_out))
                 obs_out = xp.where(done[:, None], self._normalize_obs(xp, obs_out, done), normed)
                 final_out = normed

@@ -2,7 +2,8 @@
 
 Stands where the reference puts ``gymnasium.vector.SyncVectorEnv([...partial(_init_each_env ...)])``
 (metaworld/__init__.py:460-604): same construction kwargs, same ``reset`` / ``step`` return shapes and dtypes,
-SAME_STEP autoreset with ``final_obs`` / ``final_info``, the per-env wrapper stack folded in
+SAME_STEP autoreset with ``final_obs`` / ``final_info`` (``autoreset_mode`` selects gymnasium's NEXT_STEP or DISABLED
+instead; ``reset(options={"reset_mask": m})`` resets some envs), the per-env wrapper stack folded in
 (TimeLimit, AutoTerminateOnSuccessWrapper, OneHotWrapper, RecordEpisodeStatistics,
 Random/PseudoRandomTaskSelectWrapper, CheckpointWrapper -- metaworld/wrappers.py) and the ``call`` / ``get_attr`` /
 ``set_attr`` names that ``metaworld/evaluation.py`` and the reference tests use.
@@ -41,6 +42,20 @@ def _serialize_task(task: Task) -> dict:          # metaworld/wrappers.py:35-39
 def _deserialize_task(d: dict) -> Task:            # metaworld/wrappers.py:42-47
     assert "env_name" in d and "data" in d
     return Task(env_name=d["env_name"], data=base64.b64decode(d["data"]))
+
+
+_AUTORESET_MODES = {"SameStep": "same_step", "NextStep": "next_step", "Disabled": "disabled"}
+
+
+def parse_autoreset_mode(mode):
+    """gymnasium.vector.AutoresetMode member or its value ("SameStep", "NextStep", "Disabled"; None = SAME_STEP) ->
+    that value; anything else raises ValueError."""
+    if mode is None:
+        return "SameStep"
+    v = getattr(mode, "value", mode)
+    if type(mode).__name__ == "AutoresetMode" and v in _AUTORESET_MODES or isinstance(mode, str) and mode in _AUTORESET_MODES:
+        return v
+    raise ValueError(f"autoreset_mode must be a gymnasium.vector.AutoresetMode or one of {sorted(_AUTORESET_MODES)}, got {mode!r}")
 
 
 def _rng(seed):
@@ -107,9 +122,12 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
                  env_ids=None, max_episode_steps=None, terminate_on_success=False, task_select="random",
                  reward_function_version="v2", device=0, engine=None, recurrent_info_in_obs=False,
                  normalize_reward_in_recurrent_info=True, reward_normalization_method=None, reward_alpha=0.001,
-                 normalize_observations=False, checkpoint_env_ids=None, type_seeds=None, **unused):
+                 normalize_observations=False, checkpoint_env_ids=None, type_seeds=None, autoreset_mode=None, **unused):
         if reward_function_version != "v2":
             raise NotImplementedError("only the default v2 rewards are implemented on the device")
+        # gymnasium's AutoresetMode (SyncVectorEnv): SameStep (default) / NextStep / Disabled
+        self.autoreset_mode = parse_autoreset_mode(autoreset_mode)
+        self.metadata = dict(type(self).metadata, autoreset_mode=_AUTORESET_MODES[self.autoreset_mode])
         n_types = len(env_names)
         num_envs = n_types if num_envs is None else int(num_envs)
         if num_envs < n_types:
@@ -149,6 +167,8 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             self.sub.append(_SubEnv(env_names[t_i], tasks_per_env[t_i], s, task_select != "random", eid))
         self.engine.set_envs([self._slot[e % n_types] for e in range(num_envs)])
         self._set_engine_options()
+        if self.autoreset_mode != "SameStep":
+            self.engine.set_autoreset_mode(self.autoreset_mode)
         # spaces
         T = self.num_tasks if self.use_one_hot else 0
         self.obs_dim = 39 + T
@@ -200,13 +220,19 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self._closed = False
         self._needs_reset = True
         self._device_sampler = False
+        # NEXT_STEP / DISABLED: envs whose last step ended their episode and that have not restarted (the engine's `ended`
+        # flag).  The numpy path keeps it on the host, the torch path on the device; `_ended_on_device` says where it is now
+        self._ended = np.zeros(N, dtype=bool)
+        self.d_ended = torch.zeros(N, dtype=torch.bool, device=dev)
+        self._ended_on_device = False
+        self._last_obs = self._d_last_obs = None        # what the last call returned (unmasked rows of a partial reset)
         # optional per-sub-env wrappers of the reference that sit above the one-hot wrapper (metaworld/__init__.py:437-444);
         # one instance (one set of statistics) serves both `step` and `step_torch`
         from .post import StepPost
         if recurrent_info_in_obs:
             self.obs_dtype = np.float32
         self.post = StepPost(N, recurrent_info_in_obs, normalize_reward_in_recurrent_info, reward_normalization_method, reward_alpha,
-                             normalize_observations, obs_dtype=self.obs_dtype)
+                             normalize_observations, obs_dtype=self.obs_dtype, same_step=self.autoreset_mode == "SameStep")
         if self.post.recurrent or self.post.norm_obs:
             # RNNBasedMetaRLWrapper (obs + action + reward + done, wrappers.py:55-62) and gymnasium.wrappers.NormalizeObservation
             # both declare an unbounded float32 space
@@ -267,7 +293,10 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
     # ------------------------------------------------------------------ VectorEnv API
     def reset(self, *, seed=None, options=None):
         """Every sub-env: (task-select wrapper) pick a task, then SawyerXYZEnv.reset (its `seed` argument is ignored,
-        sawyer_xyz_env.py:670)."""
+        sawyer_xyz_env.py:670).  ``options={"reset_mask": m}`` (numpy bool [num_envs], any mode) resets only the envs
+        with ``m`` set; the other rows of the returned observation are the ones the previous call returned for them."""
+        if options is not None and "reset_mask" in options:
+            return self._reset_masked(options["reset_mask"])
         N = self.num_envs
         cur = np.zeros(N, dtype=np.int32)
         for e, s in enumerate(self.sub):
@@ -284,9 +313,62 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         obs = self.h_obs.numpy().astype(self.obs_dtype)
         self._obs_template = obs.copy()        # constant columns (one-hot task id) of every later observation; see step()
         self._obs_template[:, :39] = 0
+        self._ended[:] = False
+        self._ended_on_device = False
         if self.post.active:
             obs = self.post.on_reset(obs)
+        self._last_obs, self._d_last_obs = obs, None
         return obs, {}
+
+    def _reset_masked(self, mask):
+        """gymnasium's `reset(options={"reset_mask": mask})`: the masked envs take their task-select draw and restart
+        (k_reset_masked); infos are merged for them only, and the reset info is empty."""
+        N = self.num_envs
+        assert isinstance(mask, np.ndarray), f"`options['reset_mask': mask]` must be a numpy array, got {type(mask)}"
+        assert mask.shape == (N,), f"`options['reset_mask': mask]` must have shape `({N},)`, got {mask.shape}"
+        assert mask.dtype == np.bool_, f"`options['reset_mask': mask]` must have `dtype=np.bool_`, got {mask.dtype}"
+        assert np.any(mask), f"`options['reset_mask': mask]` must contain a boolean array, got reset_mask={mask}"
+        if self._needs_reset:
+            raise RuntimeError("reset() without a mask must come first")
+        if self._device_sampler:
+            raise RuntimeError("the device-side task sampler is active (step_torch was used): use reset_torch(reset_mask) or "
+                               "disable_device_sampler() + reset()")
+        if self._last_obs is None:
+            raise RuntimeError("the last observations are on the device (step_torch): use reset_torch(reset_mask=...)")
+        self._sync_ended_to_host()
+        idx = np.nonzero(mask)[0]
+        cur = self._next_ids.copy()
+        for e in idx:
+            s = self.sub[e]
+            s.take_for_reset()
+            cur[e] = self._snap(s.current_task)
+            self._draw_pending(e)
+        t = self.torch
+        self.d_cur.copy_(t.from_numpy(cur))
+        self._push_next()
+        self.engine.reset_masked(t.from_numpy(mask).to(self.device), self.d_obs, self.d_cur)
+        self.h_obs.copy_(self.d_obs)
+        rows = self.h_obs.numpy()[idx].astype(self.obs_dtype)
+        self._ep_len[idx] = 0
+        self._ended[idx] = False
+        obs = self._last_obs.copy()
+        if self.post.active:
+            full = np.zeros((N, rows.shape[1]), dtype=self.obs_dtype)
+            full[idx] = rows
+            rows = self.post.on_reset(full, mask)[idx]
+        obs[idx] = rows
+        self._last_obs = obs
+        return obs, {}
+
+    def _sync_ended_to_host(self):
+        if self._ended_on_device:
+            self._ended = self.d_ended.cpu().numpy().copy()
+            self._ended_on_device = False
+
+    def _sync_ended_to_device(self):
+        if not self._ended_on_device:
+            self.d_ended.copy_(self.torch.from_numpy(self._ended))
+            self._ended_on_device = True
 
     def _advance_streams(self, idx):
         """The autoreset's task-select draw of sub-envs `idx` (their episode ends with this step): the speculative draw
@@ -303,6 +385,8 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         if self._device_sampler:
             raise RuntimeError("the device-side task sampler is active (step_torch was used): the numpy step API and its host "
                                "task streams are no longer in sync; call disable_device_sampler() + reset() first")
+        if self.autoreset_mode != "SameStep":
+            return self._step_deferred(actions)
         t = self.torch
         N = self.num_envs
         a = np.ascontiguousarray(actions, dtype=np.float32).reshape(N, 4)
@@ -391,6 +475,77 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             self._ep_len[idx] = 0
             if npred < len(idx):                     # terminations nobody could predict (terminate_on_success)
                 self._advance_streams(np.setdiff1d(idx, pred))
+        self._last_obs = obs
+        return obs, reward, terminated, truncated, infos
+
+    def _step_deferred(self, actions):
+        """`step` under NEXT_STEP / DISABLED autoreset (gymnasium SyncVectorEnv): the terminal step returns the terminal
+        observation and the step infos of every env, with RecordEpisodeStatistics' `episode` at the top level.  NEXT_STEP:
+        the next call restarts the envs that ended (their action is ignored) and returns their reset observation with
+        reward 0, no flags and no infos; their task-select draw becomes the running task then.  DISABLED: stepping an env
+        that ended and was not reset (`reset(options={"reset_mask": ...})`) fails before anything is launched."""
+        t = self.torch
+        N = self.num_envs
+        self._sync_ended_to_host()
+        if self.autoreset_mode == "Disabled":
+            assert not self._ended.any(), f"self._autoreset_envs={self._ended!r}"      # SyncVectorEnv's DISABLED assertion
+            restart = np.zeros(0, dtype=np.int64)
+        else:
+            restart = np.nonzero(self._ended)[0]
+        a = np.ascontiguousarray(actions, dtype=np.float32).reshape(N, 4)
+        self.h_actions.copy_(t.from_numpy(a))
+        self.d_actions.copy_(self.h_actions, non_blocking=True)
+        self.engine.step(self.d_actions, self.d_obs39, self.d_reward, self.d_term, self.d_trunc, self.d_small,
+                         self.d_final_obs39, self.d_final_info, self.d_next)
+        self.h_small.copy_(self.d_small, non_blocking=True)
+        self.h_obs39.copy_(self.d_obs39, non_blocking=True)
+        # episode returns of the predictable truncations ride with the same batch of copies (see step)
+        pred = np.nonzero((self._ep_len + 1 >= min(self.max_episode_steps, MAX_PATH_LENGTH)) & ~self._ended)[0]
+        npred = len(pred)
+        if npred:
+            self.h_idx[:npred] = t.from_numpy(pred)
+            d_pred = self.d_idx[:npred]
+            d_pred.copy_(self.h_idx[:npred], non_blocking=True)
+            self.h_final_info[:npred].copy_(self.d_final_info.index_select(0, d_pred), non_blocking=True)
+        if len(restart):                 # queued behind the kernel, which has read these envs' snapshot ids
+            self._advance_streams(restart)
+        obs = self._obs_template.copy()
+        if self.device.type == "cuda":
+            t.cuda.current_stream(self.device).synchronize()
+        np.copyto(obs[:, :39], self.h_obs39.numpy())
+        sm = np.ascontiguousarray(self.h_small.numpy().T, dtype=np.float64)
+        reward = sm[7]
+        flags = sm[8].astype(np.int8)
+        terminated, truncated = (flags & 1).astype(bool), (flags & 2).astype(bool)
+        self._ep_len += 1
+        self._ep_len[restart] = 0
+        done = terminated | truncated
+        idx = np.nonzero(done)[0]
+        infos = {}
+        if len(restart) < N:             # a restarted env's info is the (empty) reset info: value 0, mask False
+            live = np.ones(N, dtype=bool)
+            live[restart] = False
+            for i, k in enumerate(INFO_KEYS):
+                infos[k] = sm[i]
+                infos["_" + k] = live.copy()
+        ep_r = None
+        if self.post.active:
+            fresh = np.zeros(N, dtype=bool)
+            fresh[restart] = True
+            obs, reward, _, ep_r = self.post.on_step(obs, a, reward, terminated, truncated, restart=fresh)
+        if len(idx):
+            if ep_r is None:
+                if np.array_equal(idx, pred):
+                    ret = self.h_final_info[:npred, 7].numpy()
+                else:
+                    ret = self.d_final_info[:, 7].index_select(0, t.from_numpy(idx).to(self.device)).cpu().numpy()
+                ep_r = np.zeros(N)
+                ep_r[idx] = ret
+            infos["episode"] = {"r": ep_r, "l": np.where(done, self._ep_len, 0), "t": np.zeros(N),
+                                "_r": done.copy(), "_l": done.copy(), "_t": done.copy()}
+            infos["_episode"] = done.copy()
+        self._ended = done
+        self._last_obs = obs
         return obs, reward, terminated, truncated, infos
 
     def step_async(self, actions):
@@ -417,12 +572,42 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self._device_sampler = False
         self._needs_reset = True
 
-    def reset_torch(self):
-        obs, _ = self.reset()
+    def reset_torch(self, reset_mask=None):
+        """Without a mask: `reset()`, result on the device.  `reset_mask` (bool CUDA tensor [num_envs]): only those envs
+        restart, as `reset(options={"reset_mask": ...})` does, without host synchronisation: their snapshot comes from the
+        device sampler (or the pre-drawn task when no env re-samples), and the other rows are what the last
+        `step_torch` / `reset_torch` returned.  The returned tensor is overwritten by the next call."""
+        t = self.torch
+        if reset_mask is None:
+            obs, _ = self.reset()
+            if not self.post.active:
+                out = self.d_obs
+            else:        # the wrapped observation of reset(): the wrappers' statistics see the reset observation once
+                out = t.from_numpy(np.asarray(obs, dtype=np.float32)).to(self.device)
+            self._d_last_obs = out
+            return out
+        if self._needs_reset:
+            raise RuntimeError("reset_torch() without a mask must come first")
+        if not (isinstance(reset_mask, t.Tensor) and reset_mask.dtype == t.bool and reset_mask.device == self.device
+                and tuple(reset_mask.shape) == (self.num_envs,)):
+            raise ValueError(f"reset_mask must be a bool tensor of shape ({self.num_envs},) on {self.device}")
+        if not self._device_sampler and any(s.sample_tasks_on_reset for s in self.sub):
+            self.enable_device_sampler()
+        mask = reset_mask.contiguous()
+        if self._last_obs is not None and not self.post.active:      # the previous call was the numpy `reset` / `step`
+            self.d_obs.copy_(t.from_numpy(np.asarray(self._last_obs, dtype=np.float32)))
+        self.engine.reset_masked(mask, self.d_obs, None if self._device_sampler else self.d_next)
+        self._sync_ended_to_device()
+        self.d_ended &= ~mask
         if not self.post.active:
-            return self.d_obs
-        # the wrapped observation of reset(): the wrappers' statistics see the reset observation once
-        return self.torch.from_numpy(np.asarray(obs, dtype=np.float32)).to(self.device)
+            out = self.d_obs
+        else:
+            last = self._d_last_obs
+            if last is None:         # the previous call was the numpy `reset` / `step`
+                last = t.from_numpy(np.asarray(self._last_obs, dtype=np.float32)).to(self.device)
+            out = t.where(mask[:, None], self.post.on_reset(self.d_obs, mask), last)
+        self._last_obs, self._d_last_obs = None, out
+        return out
 
     def step_torch(self, actions):
         """`actions`: float32 CUDA tensor [num_envs, 4] on this env's device.  Returns device tensors (obs [N, obs_dim],
@@ -436,11 +621,20 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         if not self._device_sampler and any(s.sample_tasks_on_reset for s in self.sub):
             self.enable_device_sampler()      # without it every autoreset would restart the same pre-drawn goal
         nxt = None if self._device_sampler else self.d_next
+        restart = None
+        if self.autoreset_mode != "SameStep":      # NEXT_STEP restarts the envs that ended in the previous call
+            self._sync_ended_to_device()
+            restart = self.d_ended.clone() if self.autoreset_mode == "NextStep" else None
         self.engine.step(actions, self.d_obs, self.d_reward, self.d_term, self.d_trunc, self.d_small, self.d_final_obs,
                          self.d_final_info, nxt)
+        self._last_obs = None
+        if restart is not None or self.autoreset_mode == "Disabled":
+            t.logical_or(self.d_term, self.d_trunc, out=self.d_ended)
         if self.post.active:       # the optional wrappers on the device; the terminal observation and episode returns stay available
             obs, rew, self.d_final_obs_post, self.d_episode_return_post = self.post.on_step(
-                self.d_obs, actions, self.d_reward, self.d_term, self.d_trunc, self.d_final_obs)
+                self.d_obs, actions, self.d_reward, self.d_term, self.d_trunc,
+                self.d_final_obs if self.autoreset_mode == "SameStep" else None, restart=restart)
+            self._d_last_obs = obs
             return obs, rew, self.d_term, self.d_trunc, self.d_info
         return self.d_obs, self.d_reward, self.d_term, self.d_trunc, self.d_info
 
@@ -596,6 +790,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
                     st[e]["snapshot"] = self._snap(s.current_task)
             self.engine.set_state(st)
             self._needs_reset = False
+            self._ended, self._ended_on_device = st["ended"] != 0, False      # a run stopped between a terminal step and its restart
         if not self._needs_reset:
             for e, s in enumerate(self.sub):
                 if s.current_task is None:
@@ -613,15 +808,16 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
 
 def make_mt_envs(name, seed=None, num_tasks=None, num_envs=None, **kwargs):
     """``make_mt_envs`` (metaworld/__init__.py:460-513) -> MetaWorldVecEnv.  ``vector_strategy`` is accepted
-    and ignored (there is one strategy: the GPU).  For a task name the reference returns ONE wrapped env, not a vector
+    and ignored (there is one strategy: the GPU); ``autoreset_mode`` is gymnasium's (SAME_STEP by default).  For a task name the reference returns ONE wrapped env, not a vector
     (:470-478): pass ``single=True`` (what ``gym.make("Meta-World/MT1", ...)`` does) to get that object."""
     from . import benchmarks as B
 
     if kwargs.pop("single", False):
         from .single_env import MetaWorldSingleEnv
+        kwargs.pop("autoreset_mode", None)         # one wrapped env: no vector autoreset, as in the reference (:470-478)
         return MetaWorldSingleEnv(make_mt_envs(name, seed=seed, num_tasks=num_tasks, num_envs=1, **kwargs))
 
-    kwargs.pop("vector_strategy", None); kwargs.pop("autoreset_mode", None)
+    kwargs.pop("vector_strategy", None)
     bench = B.make_benchmark(name, seed, kwargs.pop("num_goals", B.N_GOALS))
     names = list(bench.train_classes)
     default = {"MT10": 10, "MT25": 25, "MT50": 50}.get(name, 1)
@@ -635,7 +831,7 @@ def make_ml_envs(name, seed=None, meta_batch_size=20, total_tasks_per_cls=None, 
     """``make_ml_envs`` / ``_make_ml_envs_inner`` (metaworld/__init__.py:515-604)."""
     from . import benchmarks as B
 
-    kwargs.pop("vector_strategy", None); kwargs.pop("autoreset_mode", None)
+    kwargs.pop("vector_strategy", None)
     ng = kwargs.pop("num_goals", B.N_GOALS)
     bench = B.ML1(name, seed, ng) if name in TASKS else B.make_benchmark(name, seed, ng)
     classes = list(bench.train_classes if split == "train" else bench.test_classes)
@@ -659,7 +855,7 @@ def make_custom_mt_envs(envs_list, seed=None, use_one_hot=False, num_envs=None, 
     num_tasks=len(envs_list), env_id=i, seed=seed + i)``, i.e. an MT1 benchmark of its own with its own seed."""
     from . import benchmarks as B
 
-    kwargs.pop("vector_strategy", None); kwargs.pop("autoreset_mode", None)
+    kwargs.pop("vector_strategy", None)
     ng = kwargs.pop("num_goals", B.N_GOALS)
     seeds = [None if not seed else seed + i for i in range(len(envs_list))]
     tasks = [B.MT1(n, sd, ng).train_tasks for n, sd in zip(envs_list, seeds)]
@@ -673,7 +869,7 @@ def make_custom_ml_envs(train_envs, test_envs, seed=None, meta_batch_size=20, to
 
     if set(train_envs) & set(test_envs):
         raise ValueError("The test tasks cannot contain any of the train tasks.")
-    kwargs.pop("vector_strategy", None); kwargs.pop("autoreset_mode", None)
+    kwargs.pop("vector_strategy", None)
     bench = B.Benchmark(train_envs, test_envs, True, seed, n_goals=kwargs.pop("num_goals", B.N_GOALS))
     classes = list(bench.train_classes if split == "train" else bench.test_classes)
     all_tasks = bench.train_tasks if split == "train" else bench.test_tasks
