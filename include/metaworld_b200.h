@@ -140,7 +140,8 @@ int mw_rebalance(mw_engine*);
 /* Profiling switch (default off: the timed kernel then carries no profiling atomics).  When on, mw_step additionally sums
  * the per-phase counters below, the per-model cost used by mw_rebalance, and records per env [20] u32: the 13 counters of
  * mw_get_profile for that env's last step, [13] solver iterations, [14] / [15] largest contact / constraint-row
- * count over the 6 passes, [16] launch slot (CTA), [17] convex candidate pairs queued.  Stands in for nothing in the reference (it has no profiler hook on this path).  */
+ * count over the 6 passes, [16] launch slot (CTA), [17] convex candidate pairs queued, [18] / [19] counters [13] / [14] of
+ * mw_get_profile for the convex pairs this env's warp evaluated.  Stands in for nothing in the reference (it has no profiler hook on this path).  */
 int mw_set_profiling(mw_engine*, int on);
 int mw_get_env_profile(mw_engine*, unsigned* out /*host [n_envs*20]*/);
 
@@ -148,8 +149,9 @@ int mw_get_env_profile(mw_engine*, unsigned* out /*host [n_envs*20]*/);
  * warp-cycles): [0] kinematics + mass matrix, [1] collision (incl. [2]), [2] GJK/EPA pairs, [3] constraint rows,
  * [4] bias forces + unconstrained solve, [5] constraint solver, [6] integration + glue, [7] obs / reward / autoreset,
  * [8] whole step incl. [12]; events: [9] GJK/EPA pair calls, [10] EPA expansions, [11] GJK iterations; [12] cycles spent
- * waiting for the CTA's other warps at phase boundaries (not part of [0]..[7]) */
-int mw_get_profile(mw_engine*, unsigned long long* out13);
+ * waiting for the CTA's other warps at phase boundaries (not part of [0]..[7]); [13] GJK/EPA pairs tested against their
+ * separating-axis hint, [14] of those, pairs the hint proved apart (no GJK/EPA run; [2] and [9] include them) */
+int mw_get_profile(mw_engine*, unsigned long long* out15);
 /* warp cycles each environment spent in its most recent step (host array of n_envs) */
 int mw_get_env_cost(mw_engine*, unsigned* out);
 

@@ -434,6 +434,29 @@ DEV void support_pair(const DShape& A, const DShape& B, const creal* dir, SV* o,
   support_shape(B, nd, o->b, lane);
   v3sub(o->v, o->a, o->b);
 }
+// Separating-axis hint of a general convex pair: one float4 per (env, pair) in global memory, xyz = a direction from A
+// towards B along which the pair was last proven apart, w = what convex_pair last concluded (below).  Bodies move about
+// a millimetre per substep, so an axis that separated a pair in one pass nearly always still does in the next.
+#define SEP_APART 1.f        // the last decisive "no contact" came with a separating direction
+#define SEP_HIT 2.f          // the last result was a contact: do not spend a support query on the hint
+// Returns 1 when the hint proves the pair apart by more than margin + 1e-4, 0 when it does not, -1 when there is no usable
+// hint.  Whole warp, uniform result.  The test is GJK's own separating-axis exit, with the same slack: along a unit
+// direction n, min over A - B of -n.x = -n.(support_A(n) - support_B(-n)) is a lower bound on the distance between the
+// cores, for ANY direction.  GJK's upper bound fdcore never falls below the true distance (apart from rounding at the 1e-12
+// level), so whenever this test rejects, GJK would either have left by its separating-axis test or skipped the contact at
+// `dist <= margin + 1e-4` in convex_pair: hit = 0 and no RawCon either way.  A stale, zero or garbage hint can therefore
+// only fail to reject, and nothing that is computed depends on the table's contents.
+DEV int sep_hint_test(const DShape& A, const DShape& B, creal margin, const float4* hint, int lane) {
+  const float4 h = *hint;                                 // one address for the whole warp: a broadcast load
+  if (h.w != SEP_APART) return -1;
+  creal n[3] = {h.x, h.y, h.z};
+  const creal nn = v3dot(n, n);
+  if (!(nn > (creal)1e-30 && nn < (creal)1e30)) return -1;   // zero or non-finite (NaN fails both comparisons)
+  v3scl(n, n, 1 / sqrt(nn));
+  SV w; support_pair(A, B, n, &w, lane);
+  return -v3dot(n, w.v) - core_radius(A) - core_radius(B) > margin + (creal)1e-4 ? 1 : 0;
+}
+DEV void sep_hint_store(float4* hint, const creal* n, float flag) { *hint = float4{(float)n[0], (float)n[1], (float)n[2], flag}; }
 DEV void closest_tri(const creal* a, const creal* b, const creal* c, creal* w) {
   creal ab[3], ac[3], ap[3]; v3sub(ab, b, a); v3sub(ac, c, a); v3scl(ap, a, -1);
   creal d1 = v3dot(ab, ap), d2 = v3dot(ac, ap);
@@ -698,7 +721,11 @@ DEV int cyl_cyl_parallel(const DShape& A, const DShape& B, creal margin, RawCon*
     for (int i_ = 0; i_ < n && i_ < 3; i_++) { v3addscl(fwa, fwa, s[i_].a, w4_[i_]); v3addscl(fwb, fwb, s[i_].b, w4_[i_]); } \
     creal dv_[3]; v3sub(dv_, fwb, fwa); fdcore = v3norm(dv_); \
     if (fdcore > (creal)1e-10) { outcome = 1; st = ST_DONE; } else { st = ST_G1; k = 0; } }
-__device__ __noinline__ int convex_pair(const DShape& A, const DShape& B, creal margin, RawCon* o, EpaSm* E, EpaWs* W, int lane, long long* prof = nullptr) {
+// `hint` (optional): the pair's separating-axis hint (sep_hint_test), updated by lane 0 when the result is decisive: the
+// separating direction on a "no contact" proven by an axis or by the GJK distance, SEP_HIT on a contact; left alone
+// otherwise.  It is never read here: the GJK path does not depend on it.
+__device__ __noinline__ int convex_pair(const DShape& A, const DShape& B, creal margin, RawCon* o, EpaSm* E, EpaWs* W, int lane, long long* prof = nullptr,
+                                        float4* hint = nullptr) {
   const creal dirs[6][3] = {{1, 0, 0}, {-1, 0, 0}, {0, 1, 0}, {0, -1, 0}, {0, 0, 1}, {0, 0, -1}};
   const creal ra = core_radius(A), rb = core_radius(B);
   enum { ST_GJK0 = 0, ST_GJK, ST_G1, ST_G2, ST_G3, ST_EPA, ST_DONE };
@@ -755,7 +782,10 @@ __device__ __noinline__ int convex_pair(const DShape& A, const DShape& B, creal 
       else if (st == ST_GJK) {
         const creal vw = v3dot(v, w.v);
         if (vv - vw <= (creal)1e-12 * vv || vv - vw <= GJK_TOL * sqrt(vv)) GJK_FINISH()             // |v| within GJK_TOL of the lower bound: closest point found
-        else if (vw > 0 && vw / sqrt(vv) - ra - rb > margin + (creal)1e-4) { outcome = 3; st = ST_DONE; }   // separating axis
+        else if (vw > 0 && vw / sqrt(vv) - ra - rb > margin + (creal)1e-4) {                             // separating axis
+          outcome = 3; st = ST_DONE;
+          if (hint) sep_hint_store(hint, dirl, SEP_APART);                                                  // dirl = -v: from A towards B
+        }
         else {
           bool dup = false;
           for (int i = 0; i < n; i++) { creal t[3]; v3sub(t, s[i].v, w.v); if (v3dot(t, t) < (creal)1e-24) dup = true; }
@@ -864,7 +894,7 @@ __device__ __noinline__ int convex_pair(const DShape& A, const DShape& B, creal 
         creal dvec[3]; v3sub(dvec, fwb, fwa);
         v3scl(rc.normal, dvec, 1 / fdcore); rc.dist = dist; have = true;
         v3copy(wa, fwa); v3copy(wb, fwb);
-      }
+      } else if (hint) { creal dvec[3]; v3sub(dvec, fwb, fwa); sep_hint_store(hint, dvec, SEP_APART); }
     } else if (outcome == 2 && bestf >= 0) {
       const int i0 = E->fv[0][bestf], i1 = E->fv[1][bestf], i2 = E->fv[2][bestf];
       creal w3[3]; closest_tri(E->vv[i0], E->vv[i1], E->vv[i2], w3);
@@ -877,6 +907,7 @@ __device__ __noinline__ int convex_pair(const DShape& A, const DShape& B, creal 
       for (int q = 0; q < 3; q++) rc.pos[q] = (creal)0.5 * (wa[q] + rc.normal[q] * ra + wb[q] - rc.normal[q] * rb);
       refine_cyl_box(A, B, &rc);
       result = rc.dist <= margin ? 1 : 0;
+      if (hint && result) sep_hint_store(hint, rc.normal, SEP_HIT);
     }
     if (prof) { prof[10] += eit; prof[11] += git; }
   }

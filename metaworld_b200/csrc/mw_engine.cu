@@ -43,6 +43,7 @@ struct EngineDev {
   unsigned long long* model_cycles;                  // [n_models][2]: warp cycles, env steps (drives mw_rebalance)
   unsigned* env_cost;                                // [n_envs] solver work of each env's previous step (orders the envs of a model, k_order_envs)
   unsigned* env_cycles;                              // [n_envs] cycles each env's warp spent in its previous k_step = duration of its CTA (orders the CTAs, k_order_blocks)
+  float4* sep_hint;                                  // [n_envs][MW_NCONV] separating-axis hints of the general convex pairs (k_step only; mw_collide)
   unsigned* env_prof;                                // optional [n_envs][16] per-env phase cycles / event counts of the last step (mw_set_profiling)
   int n_envs, max_steps, terminate_on_success; unsigned long long seed;
   int autoreset_mode;                                // MW_AUTORESET_* (mw_set_autoreset_mode)
@@ -91,9 +92,10 @@ DEV void stage_model(BlockShared* bs, const unsigned char* src, unsigned bytes, 
 }
 
 // wires a warp into its CTA's convex-pair queue (mw_physics.cuh: CtaShare); visible to the other warps after the first PHASE_SYNC
-DEV void join_cta(BlockShared* bs, WarpShared* wsa, WarpScratch* w, int warp, int live_warps) {
+// `sep`: the env's row of the separating-axis hint table (k_step); the other kernels run without hints
+DEV void join_cta(BlockShared* bs, WarpShared* wsa, WarpScratch* w, int warp, int live_warps, float4* sep = nullptr) {
   if (threadIdx.x == 0) { bs->cs.q_head = 0; bs->cs.nwarp = live_warps; bs->cs.peer_stride = (int)sizeof(WarpShared); bs->cs.peer0 = (unsigned char*)wsa; }
-  if ((threadIdx.x & 31) == 0) { w->cta = &bs->cs; w->warp_in_cta = warp; w->ncand = 0; w->prof_on = 0; w->nblk1 = mw_tree_split((const MwModel*)bs->model); }
+  if ((threadIdx.x & 31) == 0) { w->cta = &bs->cs; w->warp_in_cta = warp; w->ncand = 0; w->prof_on = 0; w->nblk1 = mw_tree_split((const MwModel*)bs->model); w->sep = sep; }
 #ifdef MW_CHOL_ONE_CHAIN     /* A/B switch: never split the factorisation */
   if ((threadIdx.x & 31) == 0) w->nblk1 = ((const MwModel*)bs->model)->nv;
 #endif
@@ -178,7 +180,7 @@ k_step(EngineDev e, const int* __restrict__ block_order, const int* __restrict__
   ws->w.epa = e.epa + scratch_slot(e, warp);
   ws->w.sp = e.spill + scratch_slot(e, warp);
   WarpScratch* w = &ws->w;
-  join_cta(bs, wsa, w, warp, block_count[blk]);
+  join_cta(bs, wsa, w, warp, block_count[blk], e.sep_hint + (size_t)env * MW_NCONV);
   const MwModel* m = (const MwModel*)bs->model;
   load_env(ws, e.state + env, lane);
   // NEXT_STEP / DISABLED: an env whose episode ended in the previous call still runs its physics below, so that its warp
@@ -244,7 +246,7 @@ k_step(EngineDev e, const int* __restrict__ block_order, const int* __restrict__
   }
   SYNCW();
   if (e.prof) {     // profiling runs only (mw_set_profiling): summed phase counters, per-model cost, per-env record
-    if (lane < 13) atomicAdd(e.prof + lane, (unsigned long long)w->prof[lane]);
+    if (lane < 15) atomicAdd(e.prof + lane, (unsigned long long)w->prof[lane]);
     if (lane == 0 && e.model_cycles) { atomicAdd(e.model_cycles + 2 * mi, (unsigned long long)w->prof[8]); atomicAdd(e.model_cycles + 2 * mi + 1, 1ull); }
     if (e.env_prof) {
       if (lane < 13) e.env_prof[MW_ENVPROF_W * env + lane] = (unsigned)(w->prof[lane] > 0xFFFFFFFFll ? 0xFFFFFFFFll : w->prof[lane]);
@@ -253,6 +255,7 @@ k_step(EngineDev e, const int* __restrict__ block_order, const int* __restrict__
       if (lane == 15) e.env_prof[MW_ENVPROF_W * env + 15] = (unsigned)nefc_max;
       if (lane == 16) e.env_prof[MW_ENVPROF_W * env + 16] = (unsigned)blockIdx.x;
       if (lane == 17) e.env_prof[MW_ENVPROF_W * env + 17] = (unsigned)cand_total;      // convex candidate pairs this env queued
+      if (lane == 18 || lane == 19) e.env_prof[MW_ENVPROF_W * env + lane] = (unsigned)w->prof[lane - 5];   // hint tests / rejections by this warp
     }
   }
   done = ws->info[7] != 0.f;
@@ -568,6 +571,7 @@ struct mw_engine {
   int *d_goal_first = nullptr, *d_goal_count = nullptr, *d_diag = nullptr;
   EpaWs* d_epa = nullptr; WarpSpill* d_spill = nullptr; size_t epa_cap = 0; int slot_by_sm = 0, nsmid = 0;
   unsigned long long* d_prof = nullptr; unsigned long long* d_model_cycles = nullptr; unsigned* d_env_prof = nullptr; int profiling = 0;
+  float4* d_sep_hint = nullptr;
   unsigned* d_env_cost = nullptr; unsigned* d_env_cycles = nullptr; int order_by_cycles = 1, head_warps = 0; int *d_block_order = nullptr, *d_model_first = nullptr, *d_model_count = nullptr; int n_sorted_models = 0;
   std::vector<int> h_faults;                                   // fault bits already drained from d_diag by mw_get_counters
   std::vector<int> env_model; std::vector<int> model_order;   // block table inputs (mw_rebalance re-sorts the models by measured cost)
@@ -581,6 +585,7 @@ struct mw_engine {
   EngineDev dev() const {
     EngineDev e; e.models = d_models; e.model_stride = model_stride; e.taskconsts = d_tc; e.meshverts = d_meshptrs;
     e.state = d_state; e.snaps = d_snaps; e.goal_first = d_goal_first; e.goal_count = d_goal_count; e.diag = d_diag; e.epa = d_epa; e.spill = d_spill; e.slot_by_sm = slot_by_sm; e.prof = profiling ? d_prof : nullptr; e.model_cycles = d_model_cycles; e.env_cost = d_env_cost; e.env_cycles = order_by_cycles ? d_env_cycles : nullptr; e.env_prof = profiling ? d_env_prof : nullptr;
+    e.sep_hint = d_sep_hint;
     e.n_envs = n_envs; e.max_steps = max_steps; e.terminate_on_success = terminate_on_success; e.seed = seed; e.autoreset_mode = autoreset_mode; return e;
   }
 };
@@ -742,7 +747,7 @@ void mw_destroy(mw_engine* E) {
   cudaSetDevice(E->device);
   cudaFree(E->d_models); cudaFree(E->d_tc); cudaFree(E->d_meshptrs);
   for (float* p : E->meshbufs) cudaFree(p);
-  cudaFree(E->d_state); cudaFree(E->d_snaps); cudaFree(E->d_goal_first); cudaFree(E->d_goal_count); cudaFree(E->d_diag); cudaFree(E->d_epa); cudaFree(E->d_spill); cudaFree(E->d_prof); cudaFree(E->d_model_cycles); cudaFree(E->d_env_prof); cudaFree(E->d_env_cost); cudaFree(E->d_env_cycles); cudaFree(E->d_block_order); cudaFree(E->d_model_first); cudaFree(E->d_model_count);
+  cudaFree(E->d_state); cudaFree(E->d_snaps); cudaFree(E->d_goal_first); cudaFree(E->d_goal_count); cudaFree(E->d_diag); cudaFree(E->d_epa); cudaFree(E->d_spill); cudaFree(E->d_prof); cudaFree(E->d_model_cycles); cudaFree(E->d_env_prof); cudaFree(E->d_env_cost); cudaFree(E->d_env_cycles); cudaFree(E->d_sep_hint); cudaFree(E->d_block_order); cudaFree(E->d_model_first); cudaFree(E->d_model_count);
   cudaFree(E->d_block_model); cudaFree(E->d_block_start); cudaFree(E->d_block_count); cudaFree(E->d_perm);
   cudaFree(E->d_split_head); cudaFree(E->d_split_alt); cudaFree(E->d_split_state); cudaFree(E->d_block_live);
   delete E;
@@ -763,6 +768,11 @@ int mw_set_envs(mw_engine* E, int n_envs, const int* env_model) {
   if (E->d_env_cycles) cudaFree(E->d_env_cycles);
   CK(cudaMalloc((void**)&E->d_env_cycles, sizeof(unsigned) * n_envs));
   CK(cudaMemset(E->d_env_cycles, 0, sizeof(unsigned) * n_envs));
+  // zeroed = no hint anywhere.  Never invalidated: a stale hint can only fail to reject a pair (sep_hint_test), so resets,
+  // set_state and checkpoints leave the table alone
+  if (E->d_sep_hint) cudaFree(E->d_sep_hint);
+  CK(cudaMalloc((void**)&E->d_sep_hint, sizeof(float4) * MW_NCONV * n_envs));
+  CK(cudaMemset(E->d_sep_hint, 0, sizeof(float4) * MW_NCONV * n_envs));
   if (E->d_state) cudaFree(E->d_state);
   CK(cudaMalloc((void**)&E->d_state, sizeof(MwEnvState) * n_envs));
   CK(cudaMemset(E->d_state, 0, sizeof(MwEnvState) * n_envs));
@@ -989,10 +999,10 @@ int mw_get_env_cost(mw_engine* E, unsigned* out) {
   return MW_OK;
 }
 
-int mw_get_profile(mw_engine* E, unsigned long long* out13) {
-  if (!E || !out13) return fail(MW_ERR_ARG, "mw_get_profile");
+int mw_get_profile(mw_engine* E, unsigned long long* out15) {
+  if (!E || !out15) return fail(MW_ERR_ARG, "mw_get_profile");
   CK(cudaSetDevice(E->device));
-  CK(cudaMemcpy(out13, E->d_prof, sizeof(unsigned long long) * 13, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(out15, E->d_prof, sizeof(unsigned long long) * 15, cudaMemcpyDeviceToHost));
   CK(cudaMemset(E->d_prof, 0, sizeof(unsigned long long) * 16));
   return MW_OK;
 }

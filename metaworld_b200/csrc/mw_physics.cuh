@@ -70,6 +70,7 @@ struct WarpScratch {
   alignas(16) real U[MW_UWORDS];
   EpaWs* epa;               // this warp's GJK/EPA polytope workspace (global memory, see mw_engine.cu)
   WarpSpill* sp;            // overflow storage for contacts >= MW_SMCON / rows >= MW_SMEFC (global memory)
+  float4* sep;              // this env's MW_NCONV separating-axis hints, by pair_cslot (global memory; null: no hints)
   real eD[MW_SMEFC], eAref[MW_SMEFC], eJar[MW_SMEFC], eJv[MW_SMEFC], eF[MW_SMEFC], eHd[MW_MAXSCALAR];
   Contact con[MW_SMCON];
   unsigned short cand[MW_MAXCAND];   // this env's general convex candidate pairs of the current pass (pair indices)
@@ -79,7 +80,8 @@ struct WarpScratch {
   int ncon, nefc, nscalar, nweld, solver_iter, ncon_dropped;
   int fault;                // MW_FAULT_* bits raised by the task code during this step (lane 0)
   int prof_on;              // phase timers enabled (mw_set_profiling)
-  long long prof[16];       // cycle / event counters of this step (mw_get_profile order; [12] = cycles spent waiting in PHASE_SYNC; lane 0 only)
+  long long prof[16];       // cycle / event counters of this step (mw_get_profile order; [12] = cycles spent waiting in PHASE_SYNC,
+                            // [13] / [14] = convex pairs tested against / rejected by their separating-axis hint; lane 0 only)
 };
 
 struct WarpSpill {
@@ -584,7 +586,20 @@ __device__ __noinline__ void mw_collide(const MwModel* __restrict__ m, const flo
         v3sub(t, sp, a.pos);
         r1.dist = v3dot(t, n); v3copy(r1.normal, n); v3addscl(r1.pos, sp, n, -(creal)0.5 * r1.dist);
         c1 = r1.dist <= mg;
-      } else { long long tc = MW_CLK(w); c1 = convex_pair(a, b, mg, &r1, esm, epa, lane, w->prof); if (lane == 0) { w->prof[2] += MW_CLK(w) - tc; w->prof[9] += 1; } }
+      } else {
+        const long long tc = MW_CLK(w);
+        float4* hint = nullptr;
+#ifndef MW_NO_SEPCACHE
+        if (ow->sep && m->pair_cslot[pp] < MW_NCONV) hint = ow->sep + m->pair_cslot[pp];
+#endif
+        // a pair the owner's hint still proves apart skips GJK/EPA; its result is the one GJK would give (sep_hint_test)
+        const int ht = hint ? sep_hint_test(a, b, mg, hint, lane) : -1;
+        c1 = ht == 1 ? 0 : convex_pair(a, b, mg, &r1, esm, epa, lane, w->prof, hint);
+        if (lane == 0) {
+          w->prof[2] += MW_CLK(w) - tc; w->prof[9] += 1;
+          if (w->prof_on) { w->prof[13] += ht >= 0; w->prof[14] += ht == 1; }
+        }
+      }
       if (lane == 0) { ores[k].hit = c1; if (c1) ores[k].r = r1; }
     }
   }

@@ -305,11 +305,11 @@ class Engine:
         return a[:, :ncw].reshape(self.n_envs, -1, 12), a[:, ncw:ncw + 17], a[:, ncw + 17:]
 
     PROFILE_KEYS = ["kin_mass", "collide", "gjk_epa", "constraints", "bias_smooth", "solver", "euler_glue", "obs_reward", "step",
-                    "n_convex_pairs", "n_epa_expansions", "n_gjk_iters", "barrier_wait"]
+                    "n_convex_pairs", "n_epa_expansions", "n_gjk_iters", "barrier_wait", "n_sep_tested", "n_sep_rejected"]
 
     def profile(self):
         """Per-phase warp-cycle counters summed over all env steps since the last call (mw_get_profile)."""
-        out = np.zeros(13, dtype=np.uint64)
+        out = np.zeros(len(self.PROFILE_KEYS), dtype=np.uint64)
         self.torch.cuda.synchronize(self.device)
         _ck(lib().mw_get_profile(self.h, out.ctypes.data))
         return dict(zip(self.PROFILE_KEYS, (int(x) for x in out)))
@@ -319,8 +319,8 @@ class Engine:
         _ck(lib().mw_set_profiling(self.h, int(bool(on))))
 
     def env_profile(self):
-        """[n_envs, 20] uint32: PROFILE_KEYS (13) for each env's last step, then [13] solver iterations, [14] ncon max,
-        [15] nefc max, [16] launch slot."""
+        """[n_envs, 20] uint32: the first 13 PROFILE_KEYS for each env's last step, then [13] solver iterations, [14] ncon
+        max, [15] nefc max, [16] launch slot, [17] convex pairs queued, [18] n_sep_tested, [19] n_sep_rejected."""
         out = np.zeros((self.n_envs, 20), dtype=np.uint32)
         self.torch.cuda.synchronize(self.device)
         _ck(lib().mw_get_env_profile(self.h, out.ctypes.data))

@@ -26,10 +26,13 @@ from __future__ import annotations
 import numpy as np
 
 from . import mjcf
-from .mjcf import (GEOM_MESH, GEOM_PLANE, JNT_FREE, JNT_HINGE, JNT_SLIDE, quat2mat, quat_conj, quat_mul, quat_norm)
+from .mjcf import (GEOM_BOX, GEOM_CAPSULE, GEOM_MESH, GEOM_PLANE, GEOM_SPHERE, JNT_FREE, JNT_HINGE, JNT_SLIDE, quat2mat,
+                   quat_conj, quat_mul, quat_norm)
 
 MAXLINK, MAXDOF, MAXNQ, MAXGEOM, MAXPAIR, MAXPARAM, MAXFRAME = 12, 17, 18, 40, 384, 32, 32
 NPARAM = 12
+MAXCONV = 128        # general convex pairs per model (the separating-axis hint table's row length; MT50 maximum: hammer)
+NO_CSLOT = 255       # pair_cslot of a pair that never goes to GJK/EPA
 
 # (name, ctype, shape)
 FIELDS = [
@@ -63,6 +66,7 @@ FIELDS = [
     ("geom_aabb", "f4", (MAXGEOM, 6)),      # bounding box in the geom frame: centre xyz, half extents xyz (broadphase only)
     # candidate pairs + pre-mixed contact parameters
     ("pair_g1", "u1", (MAXPAIR,)), ("pair_g2", "u1", (MAXPAIR,)), ("pair_param", "u1", (MAXPAIR,)),
+    ("pair_cslot", "u1", (MAXPAIR,)),       # slot among the model's general convex pairs (GJK/EPA candidates), else NO_CSLOT
     ("param", "f4", (MAXPARAM, NPARAM)),
     # frames read by obs / reward code
     ("frame_link", "i4", (MAXFRAME,)), ("frame_shift", "i4", (MAXFRAME,)), ("frame_pos", "f4", (MAXFRAME, 3)),
@@ -83,7 +87,8 @@ def emit_header() -> str:
     lines = ["/* GENERATED by metaworld_b200/lower.py:emit_header -- do not edit. */", "#pragma once",
              f"#define MW_MAXLINK {MAXLINK}", f"#define MW_MAXDOF {MAXDOF}", f"#define MW_MAXNQ {MAXNQ}",
              f"#define MW_MAXGEOM {MAXGEOM}", f"#define MW_MAXPAIR {MAXPAIR}", f"#define MW_MAXPARAM {MAXPARAM}",
-             f"#define MW_MAXFRAME {MAXFRAME}", f"#define MW_NPARAM {NPARAM}", "struct MwModel {"]
+             f"#define MW_MAXFRAME {MAXFRAME}", f"#define MW_NPARAM {NPARAM}", f"#define MW_NCONV {MAXCONV}",
+             "struct MwModel {"]
     for n, t, s in FIELDS:
         dims = "".join(f"[{d}]" for d in s)
         lines.append(f"  {ctype[t]} {n}{dims};")
@@ -325,13 +330,19 @@ def lower(m: mjcf.Model, movable: str | None, task_frames=()) -> Lowered:
     r["nmeshvert"] = len(out.meshvert)
 
     params = []
+    nconv = 0
     for k, (g1, g2) in enumerate(pairs):
         prm = mix_params(a, g1, g2)
         key = tuple(np.round(prm, 12))
         if key not in params:
             params.append(key)
         r["pair_g1"][k], r["pair_g2"][k], r["pair_param"][k] = cid[g1], cid[g2], params.index(key)
+        r["pair_cslot"][k] = NO_CSLOT
+        if general_convex(a["geom_type"][g1], a["geom_type"][g2]):
+            r["pair_cslot"][k] = nconv
+            nconv += 1
     assert len(params) <= MAXPARAM, len(params)
+    assert nconv <= MAXCONV, nconv
     for i, p in enumerate(params):
         r["param"][i] = p
     r["npair"] = len(pairs)
@@ -361,6 +372,14 @@ def lower(m: mjcf.Model, movable: str | None, task_frames=()) -> Lowered:
         out.frame_names.append((kind, name))
     r["nframe"] = len(frames)
     return out
+
+
+def general_convex(t1, t2) -> bool:
+    """Whether the narrowphase may send a pair (t1 <= t2) to GJK/EPA: everything but the analytic pairs (plane-*, and any
+    two of sphere / capsule / box; csrc/mw_collide.cuh pair_is_analytic) and plane-mesh, which is one support query.
+    Cylinder-box and cylinder-cylinder pairs count: they go to GJK/EPA whenever their axes are not aligned."""
+    analytic3 = (GEOM_SPHERE, GEOM_CAPSULE, GEOM_BOX)
+    return t1 != GEOM_PLANE and not (t1 in analytic3 and t2 in analytic3)
 
 
 def mix_params(a, g1, g2):

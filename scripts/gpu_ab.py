@@ -34,6 +34,11 @@ for a in acts:
     env.step_torch(a)
 e1.record(); torch.cuda.synchronize()
 N = 80
+dropped = env.engine.counters()["contacts_dropped"]
+env.engine.set_profiling(True); env.engine.profile()      # 20 profiled steps after everything compared: event counters (profile)
+for a in acts[:20]:
+    env.step_torch(a)
+prof = env.engine.profile(); env.engine.set_profiling(False)
 json.dump(dict(build=lib().mw_build_info().decode(), steps=steps, state=hashlib.sha256(st.tobytes()).hexdigest(), ms=e0.elapsed_time(e1) / (N - 20),
-               dropped=env.engine.counters()["contacts_dropped"]), open(sys.argv[1], "w"))
+               dropped=dropped, profile=prof), open(sys.argv[1], "w"))
 print("ok", sys.argv[1])
