@@ -290,6 +290,19 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             self._draw_pending(e)
         self._push_next()
 
+    def _take_reset_draws(self, idx):
+        """The task-select draw of `reset` for sub-envs `idx`: the snapshot ids of their new episodes go to `d_cur` (other
+        rows 0) and the draws for the episodes after them to `d_next`.  Each sub-env has its own RNG, so the order across
+        envs does not matter."""
+        cur = np.zeros(self.num_envs, dtype=np.int32)
+        for e in idx:
+            s = self.sub[e]
+            s.take_for_reset()
+            cur[e] = self._snap(s.current_task)
+            self._draw_pending(e)
+        self.d_cur.copy_(self.torch.from_numpy(cur))
+        self._push_next()
+
     # ------------------------------------------------------------------ VectorEnv API
     def reset(self, *, seed=None, options=None):
         """Every sub-env: (task-select wrapper) pick a task, then SawyerXYZEnv.reset (its `seed` argument is ignored,
@@ -297,15 +310,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         with ``m`` set; the other rows of the returned observation are the ones the previous call returned for them."""
         if options is not None and "reset_mask" in options:
             return self._reset_masked(options["reset_mask"])
-        N = self.num_envs
-        cur = np.zeros(N, dtype=np.int32)
-        for e, s in enumerate(self.sub):
-            s.take_for_reset()
-            cur[e] = self._snap(s.current_task)
-        for e in range(N):
-            self._draw_pending(e)
-        self.d_cur.copy_(self.torch.from_numpy(cur))
-        self._push_next()
+        self._take_reset_draws(range(self.num_envs))
         self.engine.reset(self.d_cur, self.d_obs)
         self._ep_len[:] = 0
         self._needs_reset = False
@@ -337,16 +342,8 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             raise RuntimeError("the last observations are on the device (step_torch): use reset_torch(reset_mask=...)")
         self._sync_ended_to_host()
         idx = np.nonzero(mask)[0]
-        cur = self._next_ids.copy()
-        for e in idx:
-            s = self.sub[e]
-            s.take_for_reset()
-            cur[e] = self._snap(s.current_task)
-            self._draw_pending(e)
-        t = self.torch
-        self.d_cur.copy_(t.from_numpy(cur))
-        self._push_next()
-        self.engine.reset_masked(t.from_numpy(mask).to(self.device), self.d_obs, self.d_cur)
+        self._take_reset_draws(idx)
+        self.engine.reset_masked(self.torch.from_numpy(mask).to(self.device), self.d_obs, self.d_cur)
         self.h_obs.copy_(self.d_obs)
         rows = self.h_obs.numpy()[idx].astype(self.obs_dtype)
         self._ep_len[idx] = 0
@@ -387,67 +384,25 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
                                "task streams are no longer in sync; call disable_device_sampler() + reset() first")
         if self.autoreset_mode != "SameStep":
             return self._step_deferred(actions)
-        t = self.torch
         N = self.num_envs
-        a = np.ascontiguousarray(actions, dtype=np.float32).reshape(N, 4)
-        self.h_actions.copy_(t.from_numpy(a))
-        self.d_actions.copy_(self.h_actions, non_blocking=True)
-        self.engine.step(self.d_actions, self.d_obs39, self.d_reward, self.d_term, self.d_trunc, self.d_small,
-                         self.d_final_obs39, self.d_final_info, self.d_next)
-        self.h_small.copy_(self.d_small, non_blocking=True)
-        self.h_obs39.copy_(self.d_obs39, non_blocking=True)
-        # ---- while the kernel runs: everything that does not need its results.
-        # Truncations are known in advance (the host mirrors the episode lengths): the terminal rows of those envs are
-        # fetched in the same batch of copies, their task streams are advanced and the snapshot ids of the episodes after
-        # the coming ones are queued behind the kernel (stream order: k_step reads d_next before this copy overwrites it).
-        pred = np.nonzero(self._ep_len + 1 >= min(self.max_episode_steps, MAX_PATH_LENGTH))[0]
-        npred = len(pred)
-        if npred:
-            self.h_idx[:npred] = t.from_numpy(pred)
-            d_pred = self.d_idx[:npred]
-            d_pred.copy_(self.h_idx[:npred], non_blocking=True)
-            self.h_final_obs39[:npred].copy_(self.d_final_obs39.index_select(0, d_pred), non_blocking=True)
-            self.h_final_info[:npred].copy_(self.d_final_info.index_select(0, d_pred), non_blocking=True)
+        a, pred = self._launch(actions)
+        # while the kernel runs: the task streams of the envs it truncates are advanced and the snapshot ids of the episodes
+        # after the coming ones are queued behind it (stream order: k_step reads d_next before this copy overwrites it)
+        if len(pred):
             self._advance_streams(pred)
-        # fresh arrays every step, like the reference (:637).  The array is allocated here, off the critical path, as a copy
-        # of a template that already holds the constant columns (the one-hot task id): only the 39 columns the kernel writes
-        # remain to be converted once the results are there
-        obs = self._obs_template.copy()
-        if self.device.type == "cuda":
-            t.cuda.current_stream(self.device).synchronize()
-        # ---- results (single-threaded numpy on purpose: torch's parallel host copies are faster when idle but collapse
-        # under a cgroup CPU quota smaller than the machine's core count)
-        np.copyto(obs[:, :39], self.h_obs39.numpy())
-        sm = np.ascontiguousarray(self.h_small.numpy().T, dtype=np.float64)      # [9, N]: rows are contiguous per-key arrays
-        reward = sm[7]
-        flags = sm[8].astype(np.int8)
-        terminated, truncated = (flags & 1).astype(bool), (flags & 2).astype(bool)
-        self._ep_len += 1
+        obs, sm, reward, terminated, truncated = self._collect()
         done = terminated | truncated
         idx = np.nonzero(done)[0]
         any_done = len(idx) > 0
         # SAME_STEP (gymnasium SyncVectorEnv): a finished env's step info moves to `final_info` and its slot in the
-        # top-level arrays is the (empty) reset info -> value 0, mask False; keys vanish when every env finished
-        infos = {}
-        if len(idx) < N:
-            live = ~done
-            for i, k in enumerate(INFO_KEYS):
-                v = sm[i]
-                if any_done:
-                    v[idx] = 0.0
-                infos[k] = v
-                infos["_" + k] = live.copy()
+        # top-level arrays is the (empty) reset info
+        infos = self._step_infos(sm, idx)
         fo = ep_r = None
         if any_done:
             # terminal observations / infos of the finished envs only (a few rows per step in steady state)
-            if np.array_equal(idx, pred):            # exactly the predicted truncations (always, unless success terminates)
-                rows39, rows_i = self.h_final_obs39[:npred].numpy(), self.h_final_info[:npred].numpy().copy()
-            else:
-                d_idx = t.from_numpy(idx).to(self.device, non_blocking=True)
-                rows39 = self.d_final_obs39.index_select(0, d_idx).cpu().numpy()
-                rows_i = self.d_final_info.index_select(0, d_idx).cpu().numpy()
             rows_o = self._obs_template[idx]
-            rows_o[:, :39] = rows39
+            rows_o[:, :39] = self._terminal_rows(idx, pred, self.h_final_obs39, self.d_final_obs39)
+            rows_i = self._terminal_rows(idx, pred, self.h_final_info, self.d_final_info)
         if self.post.active:
             if any_done:
                 fo = np.zeros((N, self.obs_dim), dtype=self.obs_dtype)
@@ -467,13 +422,11 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             for i, k in enumerate(INFO_KEYS):
                 final_info[k] = fi[i]                              # rows of unfinished envs are 0
                 final_info["_" + k] = done.copy()
-            final_info["episode"] = {"r": fi[7], "l": np.where(done, self._ep_len, 0),
-                                     "t": np.zeros(N), "_r": done.copy(), "_l": done.copy(), "_t": done.copy()}
-            final_info["_episode"] = done.copy()
+            final_info["episode"], final_info["_episode"] = self._episode_stats(done, fi[7])
             infos["final_obs"], infos["_final_obs"] = final_obs, done.copy()
             infos["final_info"], infos["_final_info"] = final_info, done.copy()
             self._ep_len[idx] = 0
-            if npred < len(idx):                     # terminations nobody could predict (terminate_on_success)
+            if len(pred) < len(idx):                 # terminations nobody could predict (terminate_on_success)
                 self._advance_streams(np.setdiff1d(idx, pred))
         self._last_obs = obs
         return obs, reward, terminated, truncated, infos
@@ -484,50 +437,19 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         the next call restarts the envs that ended (their action is ignored) and returns their reset observation with
         reward 0, no flags and no infos; their task-select draw becomes the running task then.  DISABLED: stepping an env
         that ended and was not reset (`reset(options={"reset_mask": ...})`) fails before anything is launched."""
-        t = self.torch
         N = self.num_envs
         self._sync_ended_to_host()
         if self.autoreset_mode == "Disabled":
             assert not self._ended.any(), f"self._autoreset_envs={self._ended!r}"      # SyncVectorEnv's DISABLED assertion
-            restart = np.zeros(0, dtype=np.int64)
-        else:
-            restart = np.nonzero(self._ended)[0]
-        a = np.ascontiguousarray(actions, dtype=np.float32).reshape(N, 4)
-        self.h_actions.copy_(t.from_numpy(a))
-        self.d_actions.copy_(self.h_actions, non_blocking=True)
-        self.engine.step(self.d_actions, self.d_obs39, self.d_reward, self.d_term, self.d_trunc, self.d_small,
-                         self.d_final_obs39, self.d_final_info, self.d_next)
-        self.h_small.copy_(self.d_small, non_blocking=True)
-        self.h_obs39.copy_(self.d_obs39, non_blocking=True)
-        # episode returns of the predictable truncations ride with the same batch of copies (see step)
-        pred = np.nonzero((self._ep_len + 1 >= min(self.max_episode_steps, MAX_PATH_LENGTH)) & ~self._ended)[0]
-        npred = len(pred)
-        if npred:
-            self.h_idx[:npred] = t.from_numpy(pred)
-            d_pred = self.d_idx[:npred]
-            d_pred.copy_(self.h_idx[:npred], non_blocking=True)
-            self.h_final_info[:npred].copy_(self.d_final_info.index_select(0, d_pred), non_blocking=True)
+        restart = np.nonzero(self._ended)[0]      # (none under DISABLED)
+        a, pred = self._launch(actions)
         if len(restart):                 # queued behind the kernel, which has read these envs' snapshot ids
             self._advance_streams(restart)
-        obs = self._obs_template.copy()
-        if self.device.type == "cuda":
-            t.cuda.current_stream(self.device).synchronize()
-        np.copyto(obs[:, :39], self.h_obs39.numpy())
-        sm = np.ascontiguousarray(self.h_small.numpy().T, dtype=np.float64)
-        reward = sm[7]
-        flags = sm[8].astype(np.int8)
-        terminated, truncated = (flags & 1).astype(bool), (flags & 2).astype(bool)
-        self._ep_len += 1
+        obs, sm, reward, terminated, truncated = self._collect()
         self._ep_len[restart] = 0
         done = terminated | truncated
         idx = np.nonzero(done)[0]
-        infos = {}
-        if len(restart) < N:             # a restarted env's info is the (empty) reset info: value 0, mask False
-            live = np.ones(N, dtype=bool)
-            live[restart] = False
-            for i, k in enumerate(INFO_KEYS):
-                infos[k] = sm[i]
-                infos["_" + k] = live.copy()
+        infos = self._step_infos(sm, restart)
         ep_r = None
         if self.post.active:
             fresh = np.zeros(N, dtype=bool)
@@ -535,18 +457,80 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             obs, reward, _, ep_r = self.post.on_step(obs, a, reward, terminated, truncated, restart=fresh)
         if len(idx):
             if ep_r is None:
-                if np.array_equal(idx, pred):
-                    ret = self.h_final_info[:npred, 7].numpy()
-                else:
-                    ret = self.d_final_info[:, 7].index_select(0, t.from_numpy(idx).to(self.device)).cpu().numpy()
                 ep_r = np.zeros(N)
-                ep_r[idx] = ret
-            infos["episode"] = {"r": ep_r, "l": np.where(done, self._ep_len, 0), "t": np.zeros(N),
-                                "_r": done.copy(), "_l": done.copy(), "_t": done.copy()}
-            infos["_episode"] = done.copy()
+                ep_r[idx] = self._terminal_rows(idx, pred, self.h_final_info[:, 7], self.d_final_info[:, 7])
+            infos["episode"], infos["_episode"] = self._episode_stats(done, ep_r)
         self._ended = done
         self._last_obs = obs
         return obs, reward, terminated, truncated, infos
+
+    def _launch(self, actions):
+        """Uploads `actions`, launches k_step and queues the copies of its results behind it: the packed [N, 9] record,
+        the 39 observation columns it writes, and the terminal rows of the envs whose episode it truncates.  Those are known
+        in advance (the host mirrors the episode lengths), so on most steps one synchronise brings back everything.
+        -> (the actions as a float32 [N, 4] array, the indices of those envs)"""
+        t = self.torch
+        a = np.ascontiguousarray(actions, dtype=np.float32).reshape(self.num_envs, 4)
+        self.h_actions.copy_(t.from_numpy(a))
+        self.d_actions.copy_(self.h_actions, non_blocking=True)
+        self.engine.step(self.d_actions, self.d_obs39, self.d_reward, self.d_term, self.d_trunc, self.d_small,
+                         self.d_final_obs39, self.d_final_info, self.d_next)
+        self.h_small.copy_(self.d_small, non_blocking=True)
+        self.h_obs39.copy_(self.d_obs39, non_blocking=True)
+        # an env that ended in the previous call (NEXT_STEP / DISABLED; none under SAME_STEP) restarts or stands still
+        pred = np.nonzero((self._ep_len + 1 >= min(self.max_episode_steps, MAX_PATH_LENGTH)) & ~self._ended)[0]
+        npred = len(pred)
+        if npred:
+            self.h_idx[:npred] = t.from_numpy(pred)
+            d_pred = self.d_idx[:npred]
+            d_pred.copy_(self.h_idx[:npred], non_blocking=True)
+            # (only SAME_STEP writes terminal observations; copying their rows in every mode keeps a single path)
+            self.h_final_obs39[:npred].copy_(self.d_final_obs39.index_select(0, d_pred), non_blocking=True)
+            self.h_final_info[:npred].copy_(self.d_final_info.index_select(0, d_pred), non_blocking=True)
+        return a, pred
+
+    def _collect(self):
+        """Waits for the step `_launch` queued and counts it in `_ep_len`.
+        -> (a fresh observation array, the packed record as [9, N] float64 rows, reward, terminated, truncated)"""
+        # fresh arrays every step, like the reference (:637).  The array is allocated before the synchronise, as a copy of
+        # a template that already holds the constant columns (the one-hot task id): only the 39 columns the kernel writes
+        # remain to be converted once the results are there
+        obs = self._obs_template.copy()
+        if self.device.type == "cuda":
+            self.torch.cuda.current_stream(self.device).synchronize()
+        # ---- results (single-threaded numpy on purpose: torch's parallel host copies are faster when idle but collapse
+        # under a cgroup CPU quota smaller than the machine's core count)
+        np.copyto(obs[:, :39], self.h_obs39.numpy())
+        sm = np.ascontiguousarray(self.h_small.numpy().T, dtype=np.float64)      # [9, N]: rows are contiguous per-key arrays
+        flags = sm[8].astype(np.int8)
+        self._ep_len += 1
+        return obs, sm, sm[7], (flags & 1).astype(bool), (flags & 2).astype(bool)
+
+    def _step_infos(self, sm, blank):
+        """The top-level step infos from the packed record's rows `sm`.  The envs `blank` report the (empty) reset info
+        instead: value 0, mask False; the keys vanish when every env does."""
+        infos = {}
+        if len(blank) < self.num_envs:
+            live = np.ones(self.num_envs, dtype=bool)
+            live[blank] = False
+            for i, k in enumerate(INFO_KEYS):
+                v = sm[i]
+                v[blank] = 0.0
+                infos[k] = v
+                infos["_" + k] = live.copy()
+        return infos
+
+    def _terminal_rows(self, idx, pred, h_rows, d_rows):
+        """Rows `idx` of the device array `d_rows`: those `_launch` copied to `h_rows` when `idx` is exactly the predicted
+        truncations `pred` (always, unless success terminates an episode), otherwise fetched now."""
+        if np.array_equal(idx, pred):
+            return h_rows[:len(pred)].numpy()
+        return d_rows.index_select(0, self.torch.from_numpy(idx).to(self.device)).cpu().numpy()
+
+    def _episode_stats(self, done, returns):
+        """RecordEpisodeStatistics' `episode` entry and `_episode` mask for the envs that finished (`done`)."""
+        return ({"r": returns, "l": np.where(done, self._ep_len, 0), "t": np.zeros(self.num_envs),
+                 "_r": done.copy(), "_l": done.copy(), "_t": done.copy()}, done.copy())
 
     def step_async(self, actions):
         self._pending_actions = actions
@@ -827,13 +811,10 @@ def make_mt_envs(name, seed=None, num_tasks=None, num_envs=None, **kwargs):
     return MetaWorldVecEnv(names, tasks, num_envs=num_envs, seed=seed, num_tasks=num_tasks or default, **kwargs)
 
 
-def make_ml_envs(name, seed=None, meta_batch_size=20, total_tasks_per_cls=None, split="train", num_envs=None, **kwargs):
-    """``make_ml_envs`` / ``_make_ml_envs_inner`` (metaworld/__init__.py:515-604)."""
-    from . import benchmarks as B
-
-    kwargs.pop("vector_strategy", None)
-    ng = kwargs.pop("num_goals", B.N_GOALS)
-    bench = B.ML1(name, seed, ng) if name in TASKS else B.make_benchmark(name, seed, ng)
+def _meta_batch(bench, split, meta_batch_size, total_tasks_per_cls):
+    """`_make_ml_envs_inner`'s meta-batch (metaworld/__init__.py:526-545): every class of the split gets `per` =
+    meta_batch_size / (number of classes) sub-envs, the i-th of them every per-th of the class's tasks from the i-th.
+    -> (env names, task lists) of the sub-envs"""
     classes = list(bench.train_classes if split == "train" else bench.test_classes)
     all_tasks = bench.train_tasks if split == "train" else bench.test_tasks
     assert meta_batch_size % len(classes) == 0, "meta_batch_size must be divisible by envs_per_task"
@@ -845,6 +826,17 @@ def make_ml_envs(name, seed=None, meta_batch_size=20, total_tasks_per_cls=None, 
             ts = ts[:total_tasks_per_cls]
         for i in range(per):
             names.append(n); tasks.append(ts[i::per])
+    return names, tasks
+
+
+def make_ml_envs(name, seed=None, meta_batch_size=20, total_tasks_per_cls=None, split="train", num_envs=None, **kwargs):
+    """``make_ml_envs`` / ``_make_ml_envs_inner`` (metaworld/__init__.py:515-604)."""
+    from . import benchmarks as B
+
+    kwargs.pop("vector_strategy", None)
+    ng = kwargs.pop("num_goals", B.N_GOALS)
+    bench = B.ML1(name, seed, ng) if name in TASKS else B.make_benchmark(name, seed, ng)
+    names, tasks = _meta_batch(bench, split, meta_batch_size, total_tasks_per_cls)
     kwargs.setdefault("task_select", "pseudorandom")
     kwargs.setdefault("checkpoint_env_ids", [None] * len(names))     # _init_each_env gets no env_id here (:548-560)
     return MetaWorldVecEnv(names, tasks, num_envs=num_envs, seed=seed, **kwargs)
@@ -871,17 +863,7 @@ def make_custom_ml_envs(train_envs, test_envs, seed=None, meta_batch_size=20, to
         raise ValueError("The test tasks cannot contain any of the train tasks.")
     kwargs.pop("vector_strategy", None)
     bench = B.Benchmark(train_envs, test_envs, True, seed, n_goals=kwargs.pop("num_goals", B.N_GOALS))
-    classes = list(bench.train_classes if split == "train" else bench.test_classes)
-    all_tasks = bench.train_tasks if split == "train" else bench.test_tasks
-    assert meta_batch_size % len(classes) == 0, "meta_batch_size must be divisible by envs_per_task"
-    per = meta_batch_size // len(classes)
-    names, tasks = [], []
-    for n in classes:
-        ts = [t for t in all_tasks if t.env_name == n]
-        if total_tasks_per_cls is not None:
-            ts = ts[:total_tasks_per_cls]
-        for i in range(per):
-            names.append(n); tasks.append(ts[i::per])
+    names, tasks = _meta_batch(bench, split, meta_batch_size, total_tasks_per_cls)
     # _make_ml_envs_inner is reached without the pseudorandom partial here: _init_each_env's default task_select="random"
     kwargs.setdefault("checkpoint_env_ids", [None] * len(names))
     return MetaWorldVecEnv(names, tasks, num_envs=num_envs, seed=seed, **kwargs)

@@ -1,7 +1,8 @@
 """CPU stand-in for `metaworld_b200.engine.Engine` backed by the float64 oracle (oracle/tasks.py): lets the REAL
 `MetaWorldVecEnv` host code run without a GPU so that its task streams, autoreset bookkeeping, info layout, episode
-statistics and checkpoints can be compared with the reference's own `gym.make_vec(...)` stack (tests/test_refpin_vector.py).
-TEST INFRASTRUCTURE: mirrors what `k_step` / `k_reset` do per environment (csrc/mw_engine.cu), nothing more."""
+statistics and checkpoints can be compared with the reference's own `gym.make_vec(...)` stack in every autoreset mode
+(tests/test_refpin_vector.py, tests/test_autoreset_modes.py).
+TEST INFRASTRUCTURE: mirrors what `k_step` / `k_reset` / `k_reset_masked` do per environment (csrc/mw_engine.cu), nothing more."""
 import numpy as np
 import torch
 
@@ -16,6 +17,7 @@ class OracleEngine:
         self.names = list(names)
         self.snaps = []           # (slot, rand_vec, partially_observable)
         self.max_steps, self.tos = 500, False
+        self.mode = "SameStep"
 
     def build_snapshots(self, mi, rvs, po, precise=None, rand_vec_pass1=None):
         first = len(self.snaps)
@@ -30,9 +32,14 @@ class OracleEngine:
         self.snap = np.zeros(self.n_envs, dtype=np.int64)
         self.plen = np.zeros(self.n_envs, dtype=np.int64)
         self.ret = np.zeros(self.n_envs)
+        self.ended = np.zeros(self.n_envs, dtype=bool)      # MwEnvState.ended
 
     def set_options(self, max_steps, tos, seed):
         self.max_steps, self.tos = int(max_steps), bool(tos)
+
+    def set_autoreset_mode(self, mode):
+        assert mode in ("SameStep", "NextStep", "Disabled")
+        self.mode = mode
 
     def set_goal_sets(self, first, count):
         raise NotImplementedError("the device sampler has no CPU stand-in")
@@ -49,7 +56,7 @@ class OracleEngine:
         o, _ = env.reset()
         if rv1 is not None:
             del env._get_state_rand_vec
-        self.snap[e], self.plen[e], self.ret[e] = sid, 0, 0.0
+        self.snap[e], self.plen[e], self.ret[e], self.ended[e] = sid, 0, 0.0, False
         return o
 
     def reset(self, snapshot_ids, obs, env_ids=None):
@@ -57,9 +64,19 @@ class OracleEngine:
         for k, e in enumerate(ids):
             obs[e, :39] = torch.from_numpy(self._start(e, int(snapshot_ids[k])).astype(np.float32))
 
+    def reset_masked(self, mask, obs, snapshot_ids=None):
+        for e in np.nonzero(mask.numpy())[0]:
+            obs[e, :39] = torch.from_numpy(self._start(e, int(snapshot_ids[e])).astype(np.float32))
+
     def step(self, actions, obs, reward, term, trunc, info, final_obs, final_info, next_snapshot):
         a = actions.numpy()
         for e, env in enumerate(self.envs):
+            if self.ended[e]:          # NEXT_STEP / DISABLED, the call after the terminal step
+                if self.mode == "Disabled":
+                    continue           # state and output rows stay as they are
+                info[e] = 0; reward[e] = 0.0; term[e] = 0; trunc[e] = 0
+                obs[e, :39] = torch.from_numpy(self._start(e, int(next_snapshot[e])).astype(np.float32))
+                continue
             o, r, _, _, inf = env.step(a[e])
             self.plen[e] += 1
             self.ret[e] += np.float32(r)
@@ -70,7 +87,10 @@ class OracleEngine:
             if info.shape[1] >= 9:
                 info[e, 7] = float(r); info[e, 8] = float(int(te) + 2 * int(tr))
             reward[e] = float(r); term[e] = int(te); trunc[e] = int(tr)
-            if te or tr:
+            if (te or tr) and self.mode != "SameStep":     # the terminal observation stays in obs, the env restarts later
+                final_info[e, 7] = float(self.ret[e])
+                self.ended[e] = True
+            elif te or tr:             # SAME_STEP autoreset
                 final_obs[e, :39] = torch.from_numpy(o.astype(np.float32))
                 final_info[e, :7] = info[e, :7]; final_info[e, 7] = float(self.ret[e])
                 o = self._start(e, int(next_snapshot[e]))
@@ -90,6 +110,7 @@ class OracleEngine:
             st[e]["target"] = np.asarray(env._target_pos, dtype=np.float32)
             if env.obj_init_pos is not None:
                 st[e]["obj_init"] = np.asarray(env.obj_init_pos, dtype=np.float32)[:3]
+        st["ended"] = self.ended
         return st
 
     def set_state(self, st):
@@ -97,3 +118,12 @@ class OracleEngine:
 
     def close(self):
         pass
+
+
+def oracle_vec_env(kind, name, **kw):
+    """`make_mt_envs` (kind "mt") or `make_ml_envs` (kind "ml") of `name` on an `OracleEngine`."""
+    from metaworld_b200 import benchmarks as B
+    from metaworld_b200 import vector_env as V
+    names = {"MT10": B.MT10, "ML10": B.ML10["train"] * 2}.get(name, [name])
+    eng = OracleEngine(list(dict.fromkeys(names)))
+    return (V.make_mt_envs if kind == "mt" else V.make_ml_envs)(name, engine=eng, **kw)

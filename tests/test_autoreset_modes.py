@@ -1,10 +1,11 @@
 """gymnasium's NEXT_STEP and DISABLED autoreset modes and `reset(options={"reset_mask": ...})`: the REAL `MetaWorldVecEnv`
-host code on the float64 oracle (tests/oracle_engine_modes.py) against the reference's own `gym.make_vec(..., autoreset_mode=...)`
+host code on the float64 oracle (tests/oracle_engine.py) against the reference's own `gym.make_vec(..., autoreset_mode=...)`
 stack, step by step.  The reference side is replayed from tests/golden/refstack_<test>.pkl.gz (tests/refstack_replay.py);
 with METAWORLD_REFERENCE=<Meta-World checkout> it runs live and rewrites those files."""
 import numpy as np
 import pytest
 
+from oracle_engine import oracle_vec_env as _ours
 from refstack_replay import RefSession
 
 KEYS = ("success", "near_object", "grasp_success", "grasp_reward", "in_place_reward", "obj_to_target", "unscaled_reward")
@@ -25,15 +26,6 @@ def gym(ref):
 @pytest.fixture
 def metaworld(ref, gym):
     return ref.module("metaworld")
-
-
-def _ours(kind, name, **kw):
-    from metaworld_b200 import vector_env as V
-    from metaworld_b200 import benchmarks as B
-    from oracle_engine_modes import OracleEngineModes as OracleEngine
-    names = {"MT10": B.MT10, "ML10": B.ML10["train"] * 2}.get(name, [name])
-    eng = OracleEngine(list(dict.fromkeys(names)))
-    return (V.make_mt_envs if kind == "mt" else V.make_ml_envs)(name, engine=eng, **kw)
 
 
 def _same_obs(o1, o2, atol):
@@ -204,7 +196,7 @@ def test_autoreset_mode_spellings_and_forwarding():
     from metaworld_b200 import entry_points
     from metaworld_b200.vector_env import parse_autoreset_mode
     from oracle.refshim.gymnasium.vector import AutoresetMode
-    from oracle_engine_modes import OracleEngineModes as OracleEngine
+    from oracle_engine import OracleEngine
     for m in AutoresetMode:
         assert parse_autoreset_mode(m) == parse_autoreset_mode(m.value) == m.value
     assert parse_autoreset_mode(None) == "SameStep"

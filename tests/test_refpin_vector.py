@@ -8,6 +8,7 @@ episode statistics, checkpoint format.  The reference side is replayed from test
 import numpy as np
 import pytest
 
+from oracle_engine import oracle_vec_env as _ours
 from refstack_replay import RefSession
 
 KEYS = ("success", "near_object", "grasp_success", "grasp_reward", "in_place_reward", "obj_to_target", "unscaled_reward")
@@ -28,15 +29,6 @@ def gym(ref):
 @pytest.fixture
 def metaworld(ref, gym):
     return ref.module("metaworld")
-
-
-def _ours(kind, name, **kw):
-    from metaworld_b200 import vector_env as V
-    from metaworld_b200 import benchmarks as B
-    from oracle_engine import OracleEngine
-    names = {"MT10": B.MT10, "ML10": B.ML10["train"] * 2}.get(name, [name])
-    eng = OracleEngine(list(dict.fromkeys(names)))
-    return (V.make_mt_envs if kind == "mt" else V.make_ml_envs)(name, engine=eng, **kw)
 
 
 def _compare_rollout(ref, ours, steps, seed, atol=2e-6):
