@@ -102,6 +102,25 @@ int mw_reset_masked(mw_engine*, const unsigned char* mask, const int* snapshot_i
  * [n,obs_stride], out DEV [n,8] = the 7 info values then the reward.                                              */
 int mw_evaluate(mw_engine*, const float* actions, const float* obs, int obs_stride, float* out, void* stream);
 
+/* MujocoEnv.set_state(qpos, qvel) (gymnasium mujoco_env.py; SawyerMocapBase.set_env_state, metaworld/sawyer_xyz_env.py:97-107)
+ * for every env with mask[i] != 0: qpos[i, :nq] and qvel[i, :nv] of that env's model become its physics state; columns
+ * past nq / nv are ignored.  qvel is ROUNDED TO FLOAT32, the type the state record keeps it in (qpos stays float64).
+ * Nothing else of the record changes: mocap, the frame stack (prev_obs), the warm-start qacc, path length, episode
+ * counters, return, target, task scalars, snapshot id and the ended mark stay as they are.  The reference's mj_forward is
+ * not run: nothing it computes outlives the next step's own forward pass (the warm start is written by the integrator
+ * only); mw_observe computes the observation of the new state.  An ended env (NEXT_STEP / DISABLED) may be set; its
+ * restart overwrites the state.  mask DEV u8 [n_envs], qpos DEV f64 [n_envs, 18], qvel DEV f64 [n_envs, 17].        */
+int mw_set_physics(mw_engine*, const unsigned char* mask, const double* qpos, const double* qvel, void* stream);
+/* SawyerMocapBase.get_env_state() (metaworld/sawyer_xyz_env.py:87-95) for every env, on the device and without host
+ * synchronisation: qpos DEV f64 [n_envs, 18], qvel DEV f64 [n_envs, 17] (the float32 record widened); columns past the
+ * env's nq / nv are zero.                                                                                         */
+int mw_get_physics(mw_engine*, double* qpos, double* qvel, void* stream);
+/* SawyerXYZEnv._get_obs() (metaworld/sawyer_xyz_env.py:513-527) of the current state for every env with mask[i] != 0:
+ * kinematics, then the frame-stacked observation, unclipped as in the reference (step() clips afterwards); like the
+ * reference it makes the current frame the env's prev_obs.  obs DEV float [n_envs, obs_stride]: row i (first 39
+ * columns) is written for the masked envs only.  A non-finite observation sets MW_FAULT_NONFINITE.                 */
+int mw_observe(mw_engine*, const unsigned char* mask, float* obs, int obs_stride, void* stream);
+
 /* Per-env fault bits accumulated since the last call (host int[n_envs], cleared by the call; synchronises).  The kernel
  * cannot raise where the reference does, so it clamps and flags:
  *   1 MW_FAULT_TOL_BOUNDS  reward_utils.tolerance: lower > upper          (ValueError, reward_utils.py:124-125)

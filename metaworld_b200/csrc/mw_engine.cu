@@ -466,6 +466,78 @@ k_evaluate(EngineDev e, const int* __restrict__ block_model, const int* __restri
   }
 }
 
+// MujocoEnv.set_state (gymnasium mujoco_env.py) without its mj_forward, one warp per env: envs with mask[env] set take
+// qpos[env, :nq] and qvel[env, :nv] of their model (qvel rounded to the record's float32); nothing else of the record
+// changes.  The forward pass is not needed: every quantity it derives is recomputed by the next step's first mw_forward
+// (or by k_observe), and the only one that outlives a pass, the warm-start qacc, is written by the integrator alone
+// (mj_Euler); the stale separating-axis hints can only fail to reject a pair (mw_set_envs)
+__global__ void k_set_physics(EngineDev e, const int* __restrict__ env_model, const unsigned char* __restrict__ mask,
+                              const double* __restrict__ qpos, const double* __restrict__ qvel) {
+  const int env = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (env >= e.n_envs || !mask[env]) return;
+  const MwModel* m = (const MwModel*)(e.models + (size_t)env_model[env] * e.model_stride);
+  if (lane < m->nq) e.state[env].qpos[lane] = qpos[(size_t)env * MW_MAXNQ + lane];
+  if (lane < m->nv) e.state[env].qvel[lane] = (float)qvel[(size_t)env * MW_MAXDOF + lane];
+}
+
+// SawyerMocapBase.get_env_state for every env: qpos [n_envs, MW_MAXNQ] float64, qvel [n_envs, MW_MAXDOF] widened to
+// float64; columns past the model's nq / nv are zero
+__global__ void k_get_physics(EngineDev e, const int* __restrict__ env_model, double* __restrict__ qpos, double* __restrict__ qvel) {
+  const int env = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (env >= e.n_envs) return;
+  const MwModel* m = (const MwModel*)(e.models + (size_t)env_model[env] * e.model_stride);
+  if (lane < MW_MAXNQ) qpos[(size_t)env * MW_MAXNQ + lane] = lane < m->nq ? e.state[env].qpos[lane] : 0.0;
+  if (lane < MW_MAXDOF) qvel[(size_t)env * MW_MAXDOF + lane] = lane < m->nv ? (double)e.state[env].qvel[lane] : 0.0;
+}
+
+// SawyerXYZEnv._get_obs (sawyer_xyz_env.py:513-527) of the current state for the envs with mask[env] set: the kinematics
+// pass, then the unclipped observation; commits prev_obs (the frame stack) like the reference.  No task's observation
+// reads contacts or forces (task_obs_objects: frame poses and qpos only), so the kinematics pass is all of mj_forward
+// that it needs.  Barriers: a CTA whose envs are all unmasked leaves before its first barrier (every thread of the CTA
+// reads the same mask bytes, so the exit is uniform); in a CTA that stays, the unmasked warps run the same kinematics
+// pass as the masked ones and so meet every barrier (the one at the start of mw_forward_kinematics_only), and only
+// skip the writes; warps past block_count exit before any barrier and are not counted by it (as in k_step).
+__global__ void __launch_bounds__(BLOCK_THREADS, 1)
+k_observe(EngineDev e, const int* __restrict__ block_model, const int* __restrict__ block_start, const int* __restrict__ block_count,
+          const int* __restrict__ perm, const unsigned char* __restrict__ mask, float* __restrict__ obs_out, int obs_stride) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  BlockShared* bs = (BlockShared*)smem;
+  WarpShared* wsa = (WarpShared*)(smem + sizeof(BlockShared));
+  {
+    bool any = false;
+    for (int k = 0; k < block_count[blockIdx.x]; k++) any = any || mask[perm[block_start[blockIdx.x] + k]];
+    if (!any) return;
+  }
+  const int mi = block_model[blockIdx.x];
+  stage_model(bs, e.models + (size_t)mi * e.model_stride, (unsigned)sizeof(bs->model), e.taskconsts + mi);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp >= block_count[blockIdx.x]) return;
+  const int env = perm[block_start[blockIdx.x] + warp];
+  WarpShared* ws = wsa + warp;
+  ws->w.epa = e.epa + scratch_slot(e, warp);
+  ws->w.sp = e.spill + scratch_slot(e, warp);
+  WarpScratch* w = &ws->w;
+  join_cta(bs, wsa, w, warp, block_count[blockIdx.x]);
+  const MwModel* m = (const MwModel*)bs->model;
+  load_env(ws, e.state + env, lane);
+  if (lane < 16) w->prof[lane] = 0;
+  if (lane == 0) { w->fault = 0; w->prof_on = 0; }
+  SYNCW();
+  mw_forward_kinematics_only(m, w, lane);
+  if (!mask[env]) return;                              // after the CTA's last barrier
+  if (lane == 0) {
+    real act[4] = {0, 0, 0, 0};
+    TaskCtx c; c.m = m; c.tc = &bs->tc; c.w = w; c.s = &ws->es; c.action = act; c.meshvert = e.meshverts[mi];
+    task_live_update(c);                               // _target_pos of the tasks that alias a site (as k_step before make_obs)
+    make_obs(c, ws->obs, /*clip=*/false);
+    bool fin = true; for (int i = 0; i < 39; i++) fin = fin && isfinite(ws->obs[i]);
+    if (!fin) e.diag[3 * env + 2] |= MW_FAULT_NONFINITE;
+  }
+  SYNCW();
+  for (int i = lane; i < 39; i += 32) obs_out[(size_t)env * obs_stride + i] = ws->obs[i];
+  ((float4*)(e.state + env))[lane] = ((const float4*)&ws->es)[lane];   // prev_obs (and a live target); the rest as loaded
+}
+
 // ---------------------------------------------------------------- launch-order maintenance
 // Environments differ several-fold in step cost (contacts, GJK/EPA, solver iterations) and a CTA holds its SM until its
 // slowest warp is done.  Cost is strongly correlated from one step to the next, so before every step (a) the envs of each
@@ -575,6 +647,7 @@ struct mw_engine {
   unsigned* d_env_cost = nullptr; unsigned* d_env_cycles = nullptr; int order_by_cycles = 1, head_warps = 0; int *d_block_order = nullptr, *d_model_first = nullptr, *d_model_count = nullptr; int n_sorted_models = 0;
   std::vector<int> h_faults;                                   // fault bits already drained from d_diag by mw_get_counters
   std::vector<int> env_model; std::vector<int> model_order;   // block table inputs (mw_rebalance re-sorts the models by measured cost)
+  int* d_env_model = nullptr;                                  // env_model on the device (k_set_physics / k_get_physics read each env's nq / nv)
   // env block table
   int n_blocks = 0; int *d_block_model = nullptr, *d_block_start = nullptr, *d_block_count = nullptr, *d_perm = nullptr;
   // head split (k_order_blocks): the alternative CTAs follow the n_blocks regular ones in the block table
@@ -733,6 +806,7 @@ int mw_create(mw_engine** out, int device, int n_models, const void* models, con
   CK(cudaFuncSetAttribute(k_snapshot, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_substeps, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_evaluate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
+  CK(cudaFuncSetAttribute(k_observe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   { const char* k = getenv("MW_B200_ORDER_KEY"); if (k && !strcmp(k, "work")) E->order_by_cycles = 0; }   // A/B switches of the launch order
   { const char* k = getenv("MW_B200_HEAD_WARPS"); if (k) E->head_warps = atoi(k); }
   { const char* k = getenv("MW_B200_SPLIT_FRAC"); if (k) E->split_frac = (float)atof(k); }
@@ -747,7 +821,7 @@ void mw_destroy(mw_engine* E) {
   cudaSetDevice(E->device);
   cudaFree(E->d_models); cudaFree(E->d_tc); cudaFree(E->d_meshptrs);
   for (float* p : E->meshbufs) cudaFree(p);
-  cudaFree(E->d_state); cudaFree(E->d_snaps); cudaFree(E->d_goal_first); cudaFree(E->d_goal_count); cudaFree(E->d_diag); cudaFree(E->d_epa); cudaFree(E->d_spill); cudaFree(E->d_prof); cudaFree(E->d_model_cycles); cudaFree(E->d_env_prof); cudaFree(E->d_env_cost); cudaFree(E->d_env_cycles); cudaFree(E->d_sep_hint); cudaFree(E->d_block_order); cudaFree(E->d_model_first); cudaFree(E->d_model_count);
+  cudaFree(E->d_state); cudaFree(E->d_snaps); cudaFree(E->d_goal_first); cudaFree(E->d_goal_count); cudaFree(E->d_diag); cudaFree(E->d_epa); cudaFree(E->d_spill); cudaFree(E->d_prof); cudaFree(E->d_model_cycles); cudaFree(E->d_env_prof); cudaFree(E->d_env_cost); cudaFree(E->d_env_cycles); cudaFree(E->d_sep_hint); cudaFree(E->d_env_model); cudaFree(E->d_block_order); cudaFree(E->d_model_first); cudaFree(E->d_model_count);
   cudaFree(E->d_block_model); cudaFree(E->d_block_start); cudaFree(E->d_block_count); cudaFree(E->d_perm);
   cudaFree(E->d_split_head); cudaFree(E->d_split_alt); cudaFree(E->d_split_state); cudaFree(E->d_block_live);
   delete E;
@@ -761,7 +835,7 @@ int mw_set_envs(mw_engine* E, int n_envs, const int* env_model) {
   E->env_model = im;
   E->n_envs = n_envs;
   E->h_faults.assign(n_envs, 0);
-  if (upload_env_blocks(E)) return MW_ERR_CUDA;
+  if (upload_env_blocks(E) || upload(&E->d_env_model, im)) return MW_ERR_CUDA;
   if (E->d_env_cost) cudaFree(E->d_env_cost);
   CK(cudaMalloc((void**)&E->d_env_cost, sizeof(unsigned) * n_envs));
   CK(cudaMemset(E->d_env_cost, 0, sizeof(unsigned) * n_envs));
@@ -890,6 +964,36 @@ int mw_evaluate(mw_engine* E, const float* actions, const float* obs, int obs_st
   if (!E || !E->d_state || !actions || !obs || !out || obs_stride < 39) return fail(MW_ERR_ARG, "mw_evaluate: bad arguments");
   CK(cudaSetDevice(E->device));
   k_evaluate<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm, actions, obs, obs_stride, out);
+  CK(cudaGetLastError());
+  E->launches++;
+  return MW_OK;
+}
+
+int mw_set_physics(mw_engine* E, const unsigned char* mask, const double* qpos, const double* qvel, void* stream) {
+  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_set_physics: mw_set_envs not called");
+  if (!mask || !qpos || !qvel) return fail(MW_ERR_ARG, "mw_set_physics: bad arguments");
+  CK(cudaSetDevice(E->device));
+  k_set_physics<<<(E->n_envs * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(E->dev(), E->d_env_model, mask, qpos, qvel);
+  CK(cudaGetLastError());
+  E->launches++;
+  return MW_OK;
+}
+
+int mw_get_physics(mw_engine* E, double* qpos, double* qvel, void* stream) {
+  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_get_physics: mw_set_envs not called");
+  if (!qpos || !qvel) return fail(MW_ERR_ARG, "mw_get_physics: bad arguments");
+  CK(cudaSetDevice(E->device));
+  k_get_physics<<<(E->n_envs * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(E->dev(), E->d_env_model, qpos, qvel);
+  CK(cudaGetLastError());
+  E->launches++;
+  return MW_OK;
+}
+
+int mw_observe(mw_engine* E, const unsigned char* mask, float* obs, int obs_stride, void* stream) {
+  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_observe: mw_set_envs not called");
+  if (!mask || !obs || obs_stride < 39) return fail(MW_ERR_ARG, "mw_observe: bad arguments");
+  CK(cudaSetDevice(E->device));
+  k_observe<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm, mask, obs, obs_stride);
   CK(cudaGetLastError());
   E->launches++;
   return MW_OK;

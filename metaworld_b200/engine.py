@@ -29,6 +29,7 @@ ENVSTATE_DTYPE = np.dtype([("qpos", "f8", 18), ("qvel", "f4", 17), ("warm", "f4"
                            ("partially_observable", "f4"), ("snapshot", "f4"), ("episode", "f4"), ("ep_return", "f4"),
                            ("ended", "f4"), ("pad", "f4", 3)])
 SNAPSHOT_DTYPE = np.dtype([("st", ENVSTATE_DTYPE), ("obs", "f4", 39), ("pad", "f4", 25)])
+MAXNQ, MAXDOF = 18, 17      # the padded qpos / qvel layout of set_physics / get_physics (ENVSTATE_DTYPE's qpos / qvel)
 INFO_KEYS = ["success", "near_object", "grasp_success", "grasp_reward", "in_place_reward", "obj_to_target",
              "unscaled_reward"]
 
@@ -67,6 +68,9 @@ def _load(path):
     L.mw_rebalance.argtypes = [vp]
     L.mw_get_env_cost.argtypes = [vp, vp]
     L.mw_evaluate.argtypes = [vp, vp, vp, ip, vp, vp]
+    L.mw_set_physics.argtypes = [vp, vp, vp, vp, vp]
+    L.mw_get_physics.argtypes = [vp, vp, vp, vp]
+    L.mw_observe.argtypes = [vp, vp, vp, ip, vp]
     L.mw_get_faults.argtypes = [vp, vp]
     L.mw_set_profiling.argtypes = [vp, ip]
     L.mw_get_env_profile.argtypes = [vp, vp]
@@ -254,6 +258,22 @@ class Engine:
     def evaluate(self, actions, obs, out):
         """evaluate_state for every env's current state: out [n, 8] = info[7], reward (mw_evaluate)."""
         _ck(lib().mw_evaluate(self.h, self._p(actions), self._p(obs), obs.stride(0), self._p(out), self._stream()))
+
+    def set_physics(self, mask, qpos, qvel):
+        """MujocoEnv.set_state for the envs with `mask` set (bool/uint8 device tensor [n_envs]): `qpos` float64 [n_envs, 18],
+        `qvel` float64 [n_envs, 17] (contiguous device tensors; columns past each model's nq / nv are ignored, qvel is
+        rounded to float32).  Changes nothing else of the state (mw_set_physics)."""
+        _ck(lib().mw_set_physics(self.h, self._p(mask), self._p(qpos), self._p(qvel), self._stream()))
+
+    def get_physics(self, qpos, qvel):
+        """Writes every env's qpos into `qpos` (float64 device tensor [n_envs, 18]) and qvel into `qvel` ([n_envs, 17]);
+        columns past nq / nv are zero (mw_get_physics)."""
+        _ck(lib().mw_get_physics(self.h, self._p(qpos), self._p(qvel), self._stream()))
+
+    def observe(self, mask, obs):
+        """_get_obs() of the current state for the envs with `mask` set, into the first 39 columns of their rows of `obs`
+        (float32 device tensor [n_envs, >= 39]); commits their frame stack (mw_observe)."""
+        _ck(lib().mw_observe(self.h, self._p(mask), self._p(obs), obs.stride(0), self._stream()))
 
     FAULTS = {1: "tolerance: lower bound > upper bound (the reference raises ValueError, reward_utils.py:124)",
               2: "tolerance: margin < 0 (the reference raises ValueError, reward_utils.py:134)",

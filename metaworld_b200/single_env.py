@@ -23,7 +23,7 @@ import numpy as np
 
 from . import _gym
 from .benchmarks import REFERENCE_CLASS, Task
-from .engine import INFO_KEYS, Engine
+from .engine import INFO_KEYS, MAXDOF, MAXNQ, Engine, lowered
 from .tasks import TASKS
 from .vector_env import MAX_PATH_LENGTH, MetaWorldVecEnv
 
@@ -182,8 +182,39 @@ class SawyerXYZEnvB200:
 
     def get_env_state(self):
         st = self._state()
-        m = self.engine.lowered[0]
-        return np.array(st["qpos"][: m.nq]), np.array(st["qvel"][: m.nv], dtype=np.float64)
+        nq, nv = self._dims()
+        return np.array(st["qpos"][:nq]), np.array(st["qvel"][:nv], dtype=np.float64)
+
+    def _dims(self):
+        rec = lowered(self.spec_).rec
+        return int(rec["nq"]), int(rec["nv"])
+
+    def set_state(self, qpos, qvel):
+        """MujocoEnv.set_state (gymnasium mujoco_env.py), with its shape assertion.  qvel is stored as float32; the frame
+        stack, mocap and task state are kept, and the observation of the new state is what `_get_obs()` returns."""
+        nq, nv = self._dims()
+        assert qpos.shape == (nq,) and qvel.shape == (nv,)
+        if not self._did_reset:
+            raise RuntimeError("reset() must be called before set_state() (the device state is created by reset)")
+        t, dev = self.torch, self.engine.device
+        q = np.zeros((1, MAXNQ)); q[0, :nq] = qpos
+        v = np.zeros((1, MAXDOF)); v[0, :nv] = qvel
+        self.engine.set_physics(t.ones(1, dtype=t.bool, device=dev), t.from_numpy(q).to(dev), t.from_numpy(v).to(dev))
+
+    def set_env_state(self, state):
+        """SawyerMocapBase.set_env_state((qpos, qvel)) (sawyer_xyz_env.py:97-107)."""
+        qpos, qvel = state
+        self.set_state(qpos, qvel)
+
+    def _get_obs(self):
+        """SawyerXYZEnv._get_obs() (sawyer_xyz_env.py:513-527): the unclipped frame-stacked observation of the current state;
+        the current frame becomes the previous one of the next step."""
+        if not self._did_reset:
+            raise RuntimeError("reset() must be called before _get_obs() (the device state is created by reset)")
+        t, dev = self.torch, self.engine.device
+        out = t.zeros(1, 39, device=dev)
+        self.engine.observe(t.ones(1, dtype=t.bool, device=dev), out)
+        return out[0].cpu().numpy().astype(np.float64)
 
     def close(self):
         if self._own_engine and self.engine is not None:

@@ -29,7 +29,7 @@ import numpy as np
 
 from . import _gym
 from .benchmarks import Task, reference_env_id
-from .engine import ENVSTATE_DTYPE, INFO_KEYS, Engine
+from .engine import ENVSTATE_DTYPE, INFO_KEYS, MAXDOF, MAXNQ, Engine, lowered
 from .tasks import TASKS
 
 MAX_PATH_LENGTH = 500     # SawyerXYZEnv.max_path_length (sawyer_xyz_env.py:152): truncates whatever TimeLimit says
@@ -191,6 +191,9 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             ids = torch.tensor([self.env_ids[e % n_types] for e in range(N)], device=dev)
             self.d_obs[torch.arange(N, device=dev), 39 + ids] = 1.0
         self.d_final_obs = self.d_obs.clone()
+        self.d_env_obs = self.d_obs.clone()            # observe_torch's output
+        self.d_all = torch.ones(N, dtype=torch.bool, device=dev)
+        self._nqnv = None
         # the numpy API's outputs: the 39 columns k_step writes, packed (stride 39): the constant one-hot columns never cross
         # the bus, and the host converts a contiguous [N, 39] block
         self.d_obs39 = torch.zeros(N, 39, device=dev)
@@ -622,6 +625,114 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             return obs, rew, self.d_term, self.d_trunc, self.d_info
         return self.d_obs, self.d_reward, self.d_term, self.d_trunc, self.d_info
 
+    # ------------------------------------------------------------------ physics state (MujocoEnv.set_state, get_env_state, _get_obs)
+    # The optional wrappers are not involved: the reference's `call` reaches these methods on the base env.
+    def _dims(self):
+        """[2, num_envs]: every env's model nq and nv."""
+        if self._nqnv is None:
+            d = {n: (int(lowered(TASKS[n]).rec["nq"]), int(lowered(TASKS[n]).rec["nv"])) for n in set(self.env_names)}
+            self._nqnv = np.array([d[s.task_name] for s in self.sub]).T
+        return self._nqnv
+
+    def _check_started(self, what):
+        if self._needs_reset:
+            raise RuntimeError(f"reset() must be called before {what} (the device state is created by reset)")
+
+    def _device_mask(self, env_mask):
+        """numpy bool [num_envs] or None (every env) -> the device tensor."""
+        if env_mask is None:
+            return self.d_all
+        m = np.asarray(env_mask)
+        if m.shape != (self.num_envs,) or m.dtype != np.bool_:
+            raise ValueError(f"env_mask must be a numpy bool array of shape ({self.num_envs},), got {m.dtype} {m.shape}")
+        return self.torch.from_numpy(m).to(self.device)
+
+    def _torch_mask(self, env_mask):
+        t = self.torch
+        if env_mask is None:
+            return self.d_all
+        if not (isinstance(env_mask, t.Tensor) and env_mask.dtype == t.bool and env_mask.device == self.device
+                and tuple(env_mask.shape) == (self.num_envs,)):
+            raise ValueError(f"env_mask must be a bool tensor of shape ({self.num_envs},) on {self.device}")
+        return env_mask.contiguous()
+
+    def set_state(self, qpos, qvel, env_mask=None):
+        """MujocoEnv.set_state for the envs with `env_mask` set (numpy bool [num_envs]; None = all): `qpos` [num_envs, 18]
+        and `qvel` [num_envs, 17] (numpy, the layout of `get_state_torch`; columns past an env's nq / nv are ignored).  qvel
+        is stored as float32.  Only the physics state changes: the observation is what `observe` computes from it, and an
+        ended env (NEXT_STEP / DISABLED) restarts from its next task as usual, overwriting the state."""
+        self._check_started("set_state")
+        N = self.num_envs
+        qpos, qvel = np.asarray(qpos, dtype=np.float64), np.asarray(qvel, dtype=np.float64)
+        if qpos.shape != (N, MAXNQ) or qvel.shape != (N, MAXDOF):
+            raise ValueError(f"set_state needs qpos of shape ({N}, {MAXNQ}) and qvel of shape ({N}, {MAXDOF}), got {qpos.shape} and {qvel.shape}")
+        mask = self._device_mask(env_mask)
+        rows = np.ones(N, dtype=bool) if env_mask is None else np.asarray(env_mask)
+        nq, nv = self._dims()
+        used_q = (np.arange(MAXNQ) < nq[:, None]) & rows[:, None]
+        used_v = (np.arange(MAXDOF) < nv[:, None]) & rows[:, None]
+        if not (np.isfinite(qpos[used_q]).all() and np.isfinite(qvel[used_v]).all()):
+            raise ValueError("set_state: qpos / qvel of the selected envs must be finite")
+        t = self.torch
+        self.engine.set_physics(mask, t.from_numpy(np.ascontiguousarray(qpos)).to(self.device),
+                                t.from_numpy(np.ascontiguousarray(qvel)).to(self.device))
+
+    def set_state_torch(self, qpos, qvel, env_mask=None):
+        """`set_state` from device tensors, without host synchronisation: `qpos` float64 [num_envs, 18], `qvel` float64
+        [num_envs, 17], contiguous, on this env's device; `env_mask` a bool tensor [num_envs] or None (all).  Values are not
+        inspected (a non-finite state shows up as a non-finite observation fault)."""
+        self._check_started("set_state_torch")
+        t = self.torch
+        for name, x, w in (("qpos", qpos, MAXNQ), ("qvel", qvel, MAXDOF)):
+            if not (isinstance(x, t.Tensor) and x.dtype == t.float64 and x.device == self.device
+                    and tuple(x.shape) == (self.num_envs, w) and x.is_contiguous()):
+                raise ValueError(f"set_state_torch needs {name} as a contiguous float64 tensor of shape ({self.num_envs}, {w}) on {self.device}")
+        self.engine.set_physics(self._torch_mask(env_mask), qpos, qvel)
+
+    def get_state_torch(self):
+        """Every env's (qpos float64 [num_envs, 18], qvel float64 [num_envs, 17]) as new device tensors, without host
+        synchronisation; columns past an env's nq / nv are zero.  `set_state_torch` takes them back."""
+        self._check_started("get_state_torch")
+        t = self.torch
+        qpos = t.empty(self.num_envs, MAXNQ, dtype=t.float64, device=self.device)
+        qvel = t.empty(self.num_envs, MAXDOF, dtype=t.float64, device=self.device)
+        self.engine.get_physics(qpos, qvel)
+        return qpos, qvel
+
+    def observe_torch(self, env_mask=None):
+        """SawyerXYZEnv._get_obs() of the current state for the envs with `env_mask` set (bool tensor [num_envs]; None =
+        all), with their one-hot columns when `use_one_hot`: the frame-stacked observation, unclipped, not passed through the
+        optional wrappers.  Like the reference it makes the current frame the env's previous one (the next step's
+        obs[18:36]).  Returns a float32 device tensor [num_envs, obs_dim] that the next call overwrites; rows of the
+        other envs are what the previous call left there (zero before the first)."""
+        self._check_started("observe_torch")
+        self.engine.observe(self._torch_mask(env_mask), self.d_env_obs)
+        return self.d_env_obs
+
+    def observe(self, env_mask=None):
+        """`observe_torch` with a numpy bool mask (None = all); a float64 numpy array [num_envs, obs_dim]."""
+        self._check_started("observe")
+        self.engine.observe(self._device_mask(env_mask), self.d_env_obs)
+        return self.d_env_obs.cpu().numpy().astype(np.float64)
+
+    def _call_set_state(self, qpos, qvel):
+        """`call("set_state", qpos, qvel)`: every sub-env's MujocoEnv.set_state with the same arrays.  Like the reference's
+        sequential calls, the envs before the first one whose nq / nv do not match the shapes are set, then that one fails
+        with MujocoEnv's AssertionError."""
+        self._check_started("set_state")
+        nq, nv = self._dims()
+        ok = [qpos.shape == (nq[e],) and qvel.shape == (nv[e],) for e in range(self.num_envs)]
+        n_ok = ok.index(False) if False in ok else self.num_envs
+        if n_ok:
+            q = np.zeros((self.num_envs, MAXNQ)); v = np.zeros((self.num_envs, MAXDOF))
+            q[:n_ok, :len(qpos)] = qpos
+            v[:n_ok, :len(qvel)] = qvel
+            mask = np.arange(self.num_envs) < n_ok
+            t = self.torch
+            self.engine.set_physics(t.from_numpy(mask).to(self.device), t.from_numpy(q).to(self.device), t.from_numpy(v).to(self.device))
+        assert n_ok == self.num_envs
+        return tuple([None] * self.num_envs)
+
     # attribute RPC used by metaworld/evaluation.py:48-169 and the reference tests
     def _current_tasks(self):
         if self._device_sampler:       # the device chose the goals: read the snapshot id of every env's running episode
@@ -688,6 +799,19 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         if name == "load_checkpoint":
             self.load_checkpoint(args[0])
             return tuple([None] * self.num_envs)
+        if name == "set_state":                 # MujocoEnv.set_state(qpos, qvel)
+            return self._call_set_state(*args, **kwargs)
+        if name == "set_env_state":             # SawyerMocapBase.set_env_state(state) (sawyer_xyz_env.py:97-107)
+            (state,) = args
+            qpos, qvel = state
+            return self._call_set_state(qpos, qvel)
+        if name == "get_env_state":             # SawyerMocapBase.get_env_state() (sawyer_xyz_env.py:87-95)
+            qpos, qvel = (x.cpu().numpy() for x in self.get_state_torch())
+            nq, nv = self._dims()
+            return tuple((qpos[e, :nq[e]].copy(), qvel[e, :nv[e]].copy()) for e in range(self.num_envs))
+        if name == "_get_obs":                  # SawyerXYZEnv._get_obs(): the base env's 39 columns
+            obs = self.observe()
+            return tuple(obs[e, :39].copy() for e in range(self.num_envs))
         return self.get_attr(name)
 
     # ------------------------------------------------------------------ checkpoint (metaworld/wrappers.py:125-142,190-204,275-322)
