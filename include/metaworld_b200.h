@@ -121,6 +121,14 @@ int mw_get_physics(mw_engine*, double* qpos, double* qvel, void* stream);
  * columns) is written for the masked envs only.  A non-finite observation sets MW_FAULT_NONFINITE.                 */
 int mw_observe(mw_engine*, const unsigned char* mask, float* obs, int obs_stride, void* stream);
 
+/* metaworld.policies (ENV_POLICY_MAP[name]().get_action(obs), metaworld/policies/__init__.py:76): the scripted expert
+ * action of every row, computed as the reference's numpy float64 code does (metaworld_b200/csrc/mw_policies.cuh) and NOT
+ * clipped.  Needs no engine: it depends on its inputs only.  task_ids DEV int32 [n] (metaworld_b200/tasks.py TASK_IDS;
+ * an id outside [0, 50) gives a NaN row), obs DEV float [n, obs_stride] (columns 0..38 are read: the base observation,
+ * one-hot columns after it are ignored), actions DEV float [n, 4].  Fails with MW_ERR_ARG for n < 0, obs_stride < 39 or
+ * a NULL pointer when n > 0.                                                                                     */
+int mw_expert_actions(const int* task_ids, const float* obs, int obs_stride, int n, float* actions, void* stream);
+
 /* Per-env fault bits accumulated since the last call (host int[n_envs], cleared by the call; synchronises).  The kernel
  * cannot raise where the reference does, so it clamps and flags:
  *   1 MW_FAULT_TOL_BOUNDS  reward_utils.tolerance: lower > upper          (ValueError, reward_utils.py:124-125)

@@ -15,6 +15,7 @@ __version__ = "0.2.0"
 
 from .benchmarks import ALL_V3, ML1, ML10, ML25, ML45, MT1, MT10, MT25, MT50, Benchmark, Task, make_benchmark  # noqa: F401
 from . import evaluation  # noqa: F401  (evaluation / metalearning_evaluation, metaworld/evaluation.py)
+from . import policies  # noqa: F401  (ENV_POLICY_MAP, the scripted expert policies, metaworld/policies/__init__.py)
 
 
 def make_mt_envs(*a, **k):

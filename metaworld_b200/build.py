@@ -18,7 +18,7 @@ NVCC_TARGET = ["-gencode", "arch=compute_90a,code=sm_90a"]
 # an env's results depended on where its constraint rows were stored.  Without contraction every build rounds each
 # operation exactly as written (DESIGN.md section 4, "Storage-independent results").
 NVCC_TARGET += ["--fmad=false"]
-HEADERS = ["mw_math.cuh", "mw_collide.cuh", "mw_physics.cuh", "mw_tasks.cuh", "mw_tasks_gen.cuh"]
+HEADERS = ["mw_math.cuh", "mw_collide.cuh", "mw_physics.cuh", "mw_tasks.cuh", "mw_tasks_gen.cuh", "mw_policies.cuh"]
 
 
 def write_header():

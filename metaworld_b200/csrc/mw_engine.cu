@@ -18,6 +18,7 @@
 
 #include "../../include/metaworld_b200.h"
 #include "mw_tasks.cuh"
+#include "mw_policies.cuh"
 
 #ifndef WARPS_PER_BLOCK
 #define WARPS_PER_BLOCK 7
@@ -488,6 +489,17 @@ __global__ void k_get_physics(EngineDev e, const int* __restrict__ env_model, do
   const MwModel* m = (const MwModel*)(e.models + (size_t)env_model[env] * e.model_stride);
   if (lane < MW_MAXNQ) qpos[(size_t)env * MW_MAXNQ + lane] = lane < m->nq ? e.state[env].qpos[lane] : 0.0;
   if (lane < MW_MAXDOF) qvel[(size_t)env * MW_MAXDOF + lane] = lane < m->nv ? (double)e.state[env].qvel[lane] : 0.0;
+}
+
+// metaworld.policies' get_action (mw_policies.cuh) for row i of a float32 observation table, one thread per row: the first
+// 39 columns widened to double, the policy of task_ids[i], the float32 action.  Reads no engine state
+__global__ void k_expert(int n, const int* __restrict__ task_ids, const float* __restrict__ obs, int obs_stride, float* __restrict__ actions) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double o[39];
+  const float* row = obs + (size_t)i * obs_stride;
+  for (int k = 0; k < 39; k++) o[k] = (double)row[k];
+  policy_action(task_ids[i], o, actions + (size_t)i * 4);
 }
 
 // SawyerXYZEnv._get_obs (sawyer_xyz_env.py:513-527) of the current state for the envs with mask[env] set: the kinematics
@@ -996,6 +1008,14 @@ int mw_observe(mw_engine* E, const unsigned char* mask, float* obs, int obs_stri
   k_observe<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm, mask, obs, obs_stride);
   CK(cudaGetLastError());
   E->launches++;
+  return MW_OK;
+}
+
+int mw_expert_actions(const int* task_ids, const float* obs, int obs_stride, int n, float* actions, void* stream) {
+  if (n < 0 || obs_stride < 39 || (n > 0 && (!task_ids || !obs || !actions))) return fail(MW_ERR_ARG, "mw_expert_actions: bad arguments");
+  if (n == 0) return MW_OK;
+  k_expert<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(n, task_ids, obs, obs_stride, actions);
+  CK(cudaGetLastError());
   return MW_OK;
 }
 

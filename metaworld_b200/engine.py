@@ -71,6 +71,7 @@ def _load(path):
     L.mw_set_physics.argtypes = [vp, vp, vp, vp, vp]
     L.mw_get_physics.argtypes = [vp, vp, vp, vp]
     L.mw_observe.argtypes = [vp, vp, vp, ip, vp]
+    L.mw_expert_actions.argtypes = [vp, vp, ip, ip, vp, vp]
     L.mw_get_faults.argtypes = [vp, vp]
     L.mw_set_profiling.argtypes = [vp, ip]
     L.mw_get_env_profile.argtypes = [vp, vp]
@@ -100,6 +101,27 @@ def lib64():
 def _ck(rc, L=None):
     if rc != 0:
         raise EngineError((L or lib()).mw_last_error().decode() or f"libmwb200 error {rc}")
+
+
+def expert_actions(task_ids, obs, out):
+    """metaworld.policies on the device (mw_expert_actions): `out[i]` = the scripted expert action of task `task_ids[i]`
+    (metaworld_b200.tasks.TASK_IDS) for observation row `obs[i, :39]`, unclipped; an unknown id gives a NaN row.  CUDA
+    tensors on one device: `task_ids` int32 [n] contiguous, `obs` float32 [n, >= 39] with contiguous rows, `out` float32
+    [n, 4] contiguous.  Asynchronous on the current stream; needs no Engine."""
+    import torch
+    n = task_ids.shape[0] if task_ids.dim() == 1 else -1
+    ok = (n >= 0 and task_ids.dtype == torch.int32 and task_ids.is_contiguous() and obs.dtype == torch.float32
+          and obs.dim() == 2 and obs.shape[0] == n and obs.shape[1] >= 39 and obs.stride(1) == 1
+          and out.dtype == torch.float32 and tuple(out.shape) == (n, 4) and out.is_contiguous()
+          and task_ids.is_cuda and obs.device == task_ids.device == out.device)
+    if not ok:
+        raise ValueError("expert_actions needs task_ids int32 [n], obs float32 [n, >= 39] (unit column stride) and out "
+                         "float32 [n, 4], contiguous, on one CUDA device")
+    with torch.cuda.device(obs.device):
+        stream = C.c_void_p(torch.cuda.current_stream(obs.device).cuda_stream)
+        _ck(lib().mw_expert_actions(C.c_void_p(task_ids.data_ptr()), C.c_void_p(obs.data_ptr()), obs.stride(0), n,
+                                    C.c_void_p(out.data_ptr()), stream))
+    return out
 
 
 _LOWERED: dict = {}

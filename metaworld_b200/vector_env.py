@@ -29,8 +29,8 @@ import numpy as np
 
 from . import _gym
 from .benchmarks import Task, reference_env_id
-from .engine import ENVSTATE_DTYPE, INFO_KEYS, MAXDOF, MAXNQ, Engine, lowered
-from .tasks import TASKS
+from .engine import ENVSTATE_DTYPE, INFO_KEYS, MAXDOF, MAXNQ, Engine, expert_actions, lowered
+from .tasks import TASK_IDS, TASKS
 
 MAX_PATH_LENGTH = 500     # SawyerXYZEnv.max_path_length (sawyer_xyz_env.py:152): truncates whatever TimeLimit says
 
@@ -197,6 +197,11 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         # the numpy API's outputs: the 39 columns k_step writes, packed (stride 39): the constant one-hot columns never cross
         # the bus, and the host converts a contiguous [N, 39] block
         self.d_obs39 = torch.zeros(N, 39, device=dev)
+        # the buffer whose first 39 columns hold every env's base observation as the last reset / step left it (before the
+        # optional wrappers): `d_obs` after `reset` and the torch calls, `d_obs39` after the numpy `step`; the default
+        # input of `expert_actions_torch`
+        self._d_raw = self.d_obs
+        self._d_expert_ids = None
         self.d_final_obs39 = torch.zeros(N, 39, device=dev)
         self.d_reward = torch.zeros(N, device=dev)
         self.d_term = torch.zeros(N, dtype=torch.uint8, device=dev)
@@ -315,6 +320,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             return self._reset_masked(options["reset_mask"])
         self._take_reset_draws(range(self.num_envs))
         self.engine.reset(self.d_cur, self.d_obs)
+        self._d_raw = self.d_obs
         self._ep_len[:] = 0
         self._needs_reset = False
         self.h_obs.copy_(self.d_obs)
@@ -346,7 +352,9 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self._sync_ended_to_host()
         idx = np.nonzero(mask)[0]
         self._take_reset_draws(idx)
-        self.engine.reset_masked(self.torch.from_numpy(mask).to(self.device), self.d_obs, self.d_cur)
+        d_mask = self.torch.from_numpy(mask).to(self.device)
+        self.engine.reset_masked(d_mask, self.d_obs, self.d_cur)
+        self._merge_raw_rows(d_mask)
         self.h_obs.copy_(self.d_obs)
         rows = self.h_obs.numpy()[idx].astype(self.obs_dtype)
         self._ep_len[idx] = 0
@@ -359,6 +367,12 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         obs[idx] = rows
         self._last_obs = obs
         return obs, {}
+
+    def _merge_raw_rows(self, d_mask):
+        """After a masked reset into `d_obs`: when the other envs' base observations are in `d_obs39` (the last call was
+        the numpy `step`), the reset rows join them there."""
+        if self._d_raw is self.d_obs39:
+            self.d_obs39.copy_(self.torch.where(d_mask[:, None], self.d_obs[:, :39], self.d_obs39))
 
     def _sync_ended_to_host(self):
         if self._ended_on_device:
@@ -478,6 +492,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self.d_actions.copy_(self.h_actions, non_blocking=True)
         self.engine.step(self.d_actions, self.d_obs39, self.d_reward, self.d_term, self.d_trunc, self.d_small,
                          self.d_final_obs39, self.d_final_info, self.d_next)
+        self._d_raw = self.d_obs39
         self.h_small.copy_(self.d_small, non_blocking=True)
         self.h_obs39.copy_(self.d_obs39, non_blocking=True)
         # an env that ended in the previous call (NEXT_STEP / DISABLED; none under SAME_STEP) restarts or stands still
@@ -584,6 +599,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         if self._last_obs is not None and not self.post.active:      # the previous call was the numpy `reset` / `step`
             self.d_obs.copy_(t.from_numpy(np.asarray(self._last_obs, dtype=np.float32)))
         self.engine.reset_masked(mask, self.d_obs, None if self._device_sampler else self.d_next)
+        self._merge_raw_rows(mask)
         self._sync_ended_to_device()
         self.d_ended &= ~mask
         if not self.post.active:
@@ -614,6 +630,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             restart = self.d_ended.clone() if self.autoreset_mode == "NextStep" else None
         self.engine.step(actions, self.d_obs, self.d_reward, self.d_term, self.d_trunc, self.d_small, self.d_final_obs,
                          self.d_final_info, nxt)
+        self._d_raw = self.d_obs
         self._last_obs = None
         if restart is not None or self.autoreset_mode == "Disabled":
             t.logical_or(self.d_term, self.d_trunc, out=self.d_ended)
@@ -714,6 +731,37 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self._check_started("observe")
         self.engine.observe(self._device_mask(env_mask), self.d_env_obs)
         return self.d_env_obs.cpu().numpy().astype(np.float64)
+
+    # ------------------------------------------------------------------ scripted experts (metaworld.policies)
+    def expert_actions_torch(self, obs=None):
+        """Every env's scripted expert action (metaworld_b200.policies: its task's policy in ENV_POLICY_MAP), as a new
+        float32 device tensor [num_envs, 4], unclipped, without host synchronisation.  `obs=None` reads each env's base
+        observation as the last `reset` / `step` / `reset_torch` / `step_torch` left it, before the optional wrappers
+        (normalisation, recurrent info), which the policies never see; on a NEXT_STEP / DISABLED terminal step that is
+        the terminal observation.  Otherwise `obs` is a float32 device tensor [num_envs, >= 39] whose first 39 columns
+        are base observations, e.g. `observe_torch()` after `set_state_torch`; later columns (one-hot ids) are ignored."""
+        t = self.torch
+        if obs is None:
+            self._check_started("expert_actions_torch")
+            obs = self._d_raw
+        elif not (isinstance(obs, t.Tensor) and obs.dtype == t.float32 and obs.device == self.device and obs.dim() == 2
+                  and obs.shape[0] == self.num_envs and obs.shape[1] >= 39 and obs.stride(1) == 1):
+            raise ValueError(f"expert_actions_torch needs obs as a float32 tensor of shape ({self.num_envs}, >= 39) with "
+                             f"contiguous rows on {self.device}")
+        if self._d_expert_ids is None:
+            self._d_expert_ids = t.tensor([TASK_IDS.get(s.task_name, -1) for s in self.sub], dtype=t.int32, device=self.device)
+        out = t.empty(self.num_envs, 4, dtype=t.float32, device=self.device)
+        expert_actions(self._d_expert_ids, obs, out)
+        return out
+
+    def expert_actions(self, obs=None):
+        """`expert_actions_torch` as a float32 numpy array [num_envs, 4]; `obs` None or a numpy array [num_envs, >= 39]."""
+        if obs is not None:
+            o = np.asarray(obs)
+            if o.ndim != 2 or o.shape[0] != self.num_envs or o.shape[1] < 39:
+                raise ValueError(f"expert_actions needs obs of shape ({self.num_envs}, >= 39), got {o.shape}")
+            obs = self.torch.from_numpy(np.ascontiguousarray(o[:, :39], dtype=np.float32)).to(self.device)
+        return self.expert_actions_torch(obs).cpu().numpy()
 
     def _call_set_state(self, qpos, qvel):
         """`call("set_state", qpos, qvel)`: every sub-env's MujocoEnv.set_state with the same arrays.  Like the reference's
