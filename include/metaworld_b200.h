@@ -121,6 +121,27 @@ int mw_get_physics(mw_engine*, double* qpos, double* qvel, void* stream);
  * columns) is written for the masked envs only.  A non-finite observation sets MW_FAULT_NONFINITE.                 */
 int mw_observe(mw_engine*, const unsigned char* mask, float* obs, int obs_stride, void* stream);
 
+/* Read-only state accessors of SawyerXYZEnv (metaworld/sawyer_xyz_env.py:67-85, 363-473, 529-535) and MujocoEnv's
+ * data.body / site / geom(name) poses, for every env with mask[i] != 0, from the env's current state.  Changes nothing:
+ * not the record (frame stack, live target), the warm start, the separating-axis hints or any fault bit other than
+ * MW_FAULT_NONFINITE (set for a non-finite frame).  Each output may be NULL; rows of unmasked envs are not written.
+ *   mask     DEV u8 [n_envs]
+ *   frame    DEV f32 [n_envs, 18] or NULL: hand position, gripper distance and the 14 object slots -- bitwise what the next
+ *            mw_observe would put into columns 0..17 (unclipped), including the live target refresh of tasks whose
+ *            _target_pos aliases a site (basketball); prev_obs is NOT committed.
+ *   frames   DEV [n_models, n_frames] 64-byte records {int link, flags; double pos[3], quat[4]} (built by
+ *            metaworld_b200/lower.py query_table from (body|site|geom, name) pairs); flags 1 = rides on the env's shift
+ *            of the task's movable body, 2 = the name is missing in that model (NaN row), 4 = the position is the env's
+ *            _target_pos (basketball's goal site), 8 / 16 = the env's _target_pos / obj_init_pos is added to the position
+ *            (sites whose model.site(name).pos reset_model sets); link -2 = relative to the mocap body.
+ *   pose     DEV f64 [n_envs, n_frames, 7] or NULL: xpos then the unit quaternion (w, x, y, z) of each named frame.
+ *   touch_geom DEV i32 [n_models] and touching DEV u8 [n_envs], both NULL or both given: touching_object(collider
+ *            touch_geom[model]) (sawyer_xyz_env.py:401-440; -1 gives 0).  With it the full mj_forward runs (contacts and
+ *            constraint forces, the fingers driven by the record's last gripper command, -1 at episode start, as
+ *            data.ctrl); without it the kinematics pass only.                                                   */
+int mw_query(mw_engine*, const unsigned char* mask, float* frame, const void* frames, int n_frames, double* pose,
+             const int* touch_geom, unsigned char* touching, void* stream);
+
 /* metaworld.policies (ENV_POLICY_MAP[name]().get_action(obs), metaworld/policies/__init__.py:76): the scripted expert
  * action of every row, computed as the reference's numpy float64 code does (metaworld_b200/csrc/mw_policies.cuh) and NOT
  * clipped.  Needs no engine: it depends on its inputs only.  task_ids DEV int32 [n] (metaworld_b200/tasks.py TASK_IDS;
@@ -145,7 +166,9 @@ int mw_set_options(mw_engine*, int max_episode_steps, int terminate_on_success, 
 int mw_set_goal_sets(mw_engine*, const int* first /*host [n_envs]*/, const int* count /*host [n_envs]*/);
 
 /* raw state access (tests, checkpoint/resume incl. physics state): n_envs * 512 bytes; record = qpos[18] float64, then
- * float32: qvel[17], warm-start qacc[17], mocap_pos[3], prev_obs[18], ... (metaworld_b200/engine.py: ENVSTATE_DTYPE) */
+ * float32: qvel[17], warm-start qacc[17], mocap_pos[3], prev_obs[18], ..., ended, gripper_ctrl (the last step's a[3],
+ * -1 in every snapshot; mw_set_physics leaves it alone; a record saved before the field existed holds 0 there, which
+ * only mw_query's touching reads, until the next step), pad[2] (metaworld_b200/engine.py: ENVSTATE_DTYPE)          */
 int mw_get_state(mw_engine*, void* out_host);
 int mw_set_state(mw_engine*, const void* in_host);
 /* debug: run nstep raw physics substeps (mj_step) on every env with fixed ctrl, no reward/obs */

@@ -278,6 +278,7 @@ k_step(EngineDev e, const int* __restrict__ block_order, const int* __restrict__
         if (final_info && lane == 7) final_info[(size_t)env * 8 + 7] = ws->es.ep_return;
         if (lane == 0) ws->es.ended = 1.f;
       }
+      if (lane == 0) ws->es.gripper_ctrl = actions[4 * env + 3];   // data.ctrl of this state (k_query's contact forces)
       for (int i = lane; i < 39; i += 32) obs_out[(size_t)env * obs_stride + i] = ws->obs[i];
       store_env(ws, e.state + env, lane);
       return;
@@ -354,6 +355,7 @@ k_snapshot(EngineDev e, const int* __restrict__ block_model, const int* __restri
     make_obs(c, ws->obs, false);                       // _get_obs() of pass 2, not clipped
     for (int i = 0; i < 18; i++) { ws->obs[18 + i] = ws->obs[i]; }   // reset(): obs[18:36] = obs[:18]  (:679-680)
     ws->es.path_len = 0.f; ws->es.episode = 0.f; ws->es.ep_return = 0.f; ws->es.snapshot = (float)(snap_base + item);
+    ws->es.gripper_ctrl = -1.f;                        // _reset_hand leaves ctrl = [-1, 1]
   }
   SYNCW();
   if (lane < 3) ws->es.shift[lane] = (float)w->shift[lane];
@@ -548,6 +550,97 @@ k_observe(EngineDev e, const int* __restrict__ block_model, const int* __restric
   SYNCW();
   for (int i = lane; i < 39; i += 32) obs_out[(size_t)env * obs_stride + i] = ws->obs[i];
   ((float4*)(e.state + env))[lane] = ((const float4*)&ws->es)[lane];   // prev_obs (and a live target); the rest as loaded
+}
+
+// one named frame of a query table (mw_query; built by metaworld_b200/lower.py query_table): the pose relative to link
+// `link`, to the world when link == -1 (translated by the env's shift when MW_QF_SHIFT), or to the mocap body when
+// link == MW_QF_MOCAP_LINK
+#define MW_QF_SHIFT 1       // a static frame that rides on the task's movable body (model.body(..).pos edits)
+#define MW_QF_MISSING 2     // the name does not exist in this model: NaN row
+#define MW_QF_TARGET 4      // the position is the env's _target_pos (a site the task keeps aliased to it: basketball's goal)
+#define MW_QF_MOCAP_LINK -2 // the frame rides on the mocap body (data.mocap_pos, mocap_quat)
+#define MW_QF_ADD_TARGET 8  // a site whose model.site(..).pos reset_model set to _target_pos: + the env's target
+#define MW_QF_ADD_OBJ_INIT 16   // the same with obj_init_pos (disassemble's pegTop)
+struct MwQueryFrame { int link, flags; double pos[3], quat[4]; };
+static_assert(sizeof(MwQueryFrame) == 64, "MwQueryFrame layout mismatch with lower.py QUERY_DTYPE");
+
+// Read-only state query of the envs with mask[env] set (mw_query): the current observation frame (columns 0..17 of the next
+// _get_obs, unclipped), world poses of named frames and touching_object of one collider.  Nothing is written back: not the
+// record (the frame stack, the live target), the warm start, the separating-axis hints (join_cta without hints) or any fault
+// bit but MW_FAULT_NONFINITE.  Barriers as in k_observe: a CTA without a masked env leaves before its first barrier, the
+// unmasked warps of a CTA that stays run the same pass and skip the writes, warps past block_count exit before any barrier.
+// `touch_geom` non-null: the full forward pass (contacts, constraint forces from the record's gripper command), else the
+// kinematics pass only.
+__global__ void __launch_bounds__(BLOCK_THREADS, 1)
+k_query(EngineDev e, const int* __restrict__ block_model, const int* __restrict__ block_start, const int* __restrict__ block_count,
+        const int* __restrict__ perm, const unsigned char* __restrict__ mask, float* __restrict__ frame_out,
+        const MwQueryFrame* __restrict__ table, int nq_frames, double* __restrict__ pose_out,
+        const int* __restrict__ touch_geom, unsigned char* __restrict__ touching_out) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  BlockShared* bs = (BlockShared*)smem;
+  WarpShared* wsa = (WarpShared*)(smem + sizeof(BlockShared));
+  {
+    bool any = false;
+    for (int k = 0; k < block_count[blockIdx.x]; k++) any = any || mask[perm[block_start[blockIdx.x] + k]];
+    if (!any) return;
+  }
+  const int mi = block_model[blockIdx.x];
+  stage_model(bs, e.models + (size_t)mi * e.model_stride, (unsigned)sizeof(bs->model), e.taskconsts + mi);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp >= block_count[blockIdx.x]) return;
+  const int env = perm[block_start[blockIdx.x] + warp];
+  WarpShared* ws = wsa + warp;
+  ws->w.epa = e.epa + scratch_slot(e, warp);
+  ws->w.sp = e.spill + scratch_slot(e, warp);
+  WarpScratch* w = &ws->w;
+  join_cta(bs, wsa, w, warp, block_count[blockIdx.x]);
+  const MwModel* m = (const MwModel*)bs->model;
+  load_env(ws, e.state + env, lane);
+  if (lane < 16) w->prof[lane] = 0;
+  if (lane == 0) { w->fault = 0; w->prof_on = 0; w->ctrl[0] = ws->es.gripper_ctrl; w->ctrl[1] = -ws->es.gripper_ctrl; }
+  SYNCW();
+  if (touching_out) mw_forward(m, e.meshverts[mi], w, lane);
+  else mw_forward_kinematics_only(m, w, lane);
+  if (!mask[env]) return;                              // after the CTA's last barrier
+  real act[4] = {0, 0, 0, 0};
+  TaskCtx c; c.m = m; c.tc = &bs->tc; c.w = w; c.s = &ws->es; c.action = act; c.meshvert = e.meshverts[mi];
+  if (lane == 0) {
+    task_live_update(c);                               // basketball's aliased goal, as before make_obs in k_step
+    if (frame_out) {
+      make_obs(c, ws->obs, /*clip=*/false);            // also advances ws->es.prev_obs, which is never stored
+      bool fin = true; for (int i = 0; i < 18; i++) fin = fin && isfinite(ws->obs[i]);
+      if (!fin) e.diag[3 * env + 2] |= MW_FAULT_NONFINITE;
+    }
+    if (touching_out) { const int g = touch_geom[mi]; touching_out[env] = g >= 0 && touching_object(c, g, (int)bs->tc.p[14], (int)bs->tc.p[15]); }
+  }
+  SYNCW();
+  if (frame_out) for (int i = lane; i < 18; i += 32) frame_out[(size_t)env * 18 + i] = ws->obs[i];
+  if (pose_out) {
+    for (int k = lane; k < nq_frames; k += 32) {       // one frame per lane, in float64 from the float64 link poses
+      const MwQueryFrame f = table[(size_t)mi * nq_frames + k];
+      double* o = pose_out + ((size_t)env * nq_frames + k) * 7;
+      if (f.flags & MW_QF_MISSING) { for (int i = 0; i < 7; i++) o[i] = __longlong_as_double(0x7ff8000000000000ll); continue; }
+      double p[3], q[4];
+      if (f.link == -1) {
+        for (int i = 0; i < 3; i++) p[i] = f.pos[i] + ((f.flags & MW_QF_SHIFT) ? (double)w->shift[i] : 0.0);
+        for (int i = 0; i < 4; i++) q[i] = f.quat[i];
+      } else {
+        const bool mocap = f.link == MW_QF_MOCAP_LINK;
+        double R[9], lq[4], lp[3], t[3];
+        for (int i = 0; i < 4; i++) lq[i] = mocap ? (double)w->mocap_quat[i] : w->lquatd[f.link][i];
+        for (int i = 0; i < 3; i++) lp[i] = mocap ? (double)w->mocap_pos[i] : w->lposd[f.link][i];
+        if (mocap) quat_normalize(lq);
+        quat2mat(R, lq); mat_mulvec(t, R, f.pos); v3add(p, lp, t);
+        quat_mul(q, lq, f.quat);
+      }
+      quat_normalize(q);
+      if (f.flags & MW_QF_ADD_TARGET) for (int i = 0; i < 3; i++) p[i] += (double)ws->es.target[i];
+      if (f.flags & MW_QF_ADD_OBJ_INIT) for (int i = 0; i < 3; i++) p[i] += (double)ws->es.obj_init[i];
+      if (f.flags & MW_QF_TARGET) for (int i = 0; i < 3; i++) p[i] = ws->es.target[i];
+      for (int i = 0; i < 3; i++) o[i] = p[i];
+      for (int i = 0; i < 4; i++) o[3 + i] = q[i];
+    }
+  }
 }
 
 // ---------------------------------------------------------------- launch-order maintenance
@@ -819,6 +912,7 @@ int mw_create(mw_engine** out, int device, int n_models, const void* models, con
   CK(cudaFuncSetAttribute(k_substeps, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_evaluate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_observe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
+  CK(cudaFuncSetAttribute(k_query, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   { const char* k = getenv("MW_B200_ORDER_KEY"); if (k && !strcmp(k, "work")) E->order_by_cycles = 0; }   // A/B switches of the launch order
   { const char* k = getenv("MW_B200_HEAD_WARPS"); if (k) E->head_warps = atoi(k); }
   { const char* k = getenv("MW_B200_SPLIT_FRAC"); if (k) E->split_frac = (float)atof(k); }
@@ -1006,6 +1100,20 @@ int mw_observe(mw_engine* E, const unsigned char* mask, float* obs, int obs_stri
   if (!mask || !obs || obs_stride < 39) return fail(MW_ERR_ARG, "mw_observe: bad arguments");
   CK(cudaSetDevice(E->device));
   k_observe<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm, mask, obs, obs_stride);
+  CK(cudaGetLastError());
+  E->launches++;
+  return MW_OK;
+}
+
+int mw_query(mw_engine* E, const unsigned char* mask, float* frame, const void* frames, int n_frames, double* pose,
+             const int* touch_geom, unsigned char* touching, void* stream) {
+  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_query: mw_set_envs not called");
+  if (!mask || n_frames < 0 || (pose && (!frames || n_frames == 0)) || (!touching) != (!touch_geom))
+    return fail(MW_ERR_ARG, "mw_query: bad arguments");
+  if (!frame && !pose && !touching) return MW_OK;
+  CK(cudaSetDevice(E->device));
+  k_query<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm,
+      mask, frame, (const MwQueryFrame*)frames, pose ? n_frames : 0, pose, touch_geom, touching);
   CK(cudaGetLastError());
   E->launches++;
   return MW_OK;

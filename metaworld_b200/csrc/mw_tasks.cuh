@@ -26,7 +26,8 @@ struct MwEnvState {
   float episode;             // episodes completed (drives the device-side task sampler)
   float ep_return;
   float ended;               // 1: the last step ended the episode and the env has not restarted (NEXT_STEP / DISABLED autoreset)
-  float pad[3];
+  float gripper_ctrl;        // last gripper command a[3] (data.ctrl = [a3, -a3]); -1 at episode start (_reset_hand)
+  float pad[2];
 };
 static_assert(sizeof(MwEnvState) == 128 * 4, "MwEnvState must be 128 floats");
 

@@ -12,7 +12,7 @@ import os
 import numpy as np
 
 from . import lower, modelzoo
-from .tasks import TASKS, TaskSpec
+from .tasks import MOVED_SITES, TARGET_ALIAS, TASKS, TaskSpec
 
 _LIB = None
 _LIB64 = None
@@ -27,7 +27,7 @@ ENVSTATE_DTYPE = np.dtype([("qpos", "f8", 18), ("qvel", "f4", 17), ("warm", "f4"
                            ("prev_obs", "f4", 18), ("shift", "f4", 3), ("target", "f4", 3), ("obj_init", "f4", 3),
                            ("init_tcp", "f4", 3), ("scal", "f4", 16), ("path_len", "f4"),
                            ("partially_observable", "f4"), ("snapshot", "f4"), ("episode", "f4"), ("ep_return", "f4"),
-                           ("ended", "f4"), ("pad", "f4", 3)])
+                           ("ended", "f4"), ("gripper_ctrl", "f4"), ("pad", "f4", 2)])
 SNAPSHOT_DTYPE = np.dtype([("st", ENVSTATE_DTYPE), ("obs", "f4", 39), ("pad", "f4", 25)])
 MAXNQ, MAXDOF = 18, 17      # the padded qpos / qvel layout of set_physics / get_physics (ENVSTATE_DTYPE's qpos / qvel)
 INFO_KEYS = ["success", "near_object", "grasp_success", "grasp_reward", "in_place_reward", "obj_to_target",
@@ -72,6 +72,7 @@ def _load(path):
     L.mw_get_physics.argtypes = [vp, vp, vp, vp]
     L.mw_observe.argtypes = [vp, vp, vp, ip, vp]
     L.mw_expert_actions.argtypes = [vp, vp, ip, ip, vp, vp]
+    L.mw_query.argtypes = [vp, vp, vp, vp, ip, vp, vp, vp, vp]
     L.mw_get_faults.argtypes = [vp, vp]
     L.mw_set_profiling.argtypes = [vp, ip]
     L.mw_get_env_profile.argtypes = [vp, vp]
@@ -181,6 +182,7 @@ class Engine:
                             nmv.ctypes.data))
         self.h64 = None
         self.n_envs = 0
+        self._query_tables = {}      # device copies of the mw_query tables, by frame list / geom list
 
     def close(self):
         if getattr(self, "h64", None):
@@ -296,6 +298,34 @@ class Engine:
         """_get_obs() of the current state for the envs with `mask` set, into the first 39 columns of their rows of `obs`
         (float32 device tensor [n_envs, >= 39]); commits their frame stack (mw_observe)."""
         _ck(lib().mw_observe(self.h, self._p(mask), self._p(obs), obs.stride(0), self._stream()))
+
+    def query(self, mask, frame=None, pose=None, frames=None, touching=None, main_geom=None):
+        """Read-only accessors of the current state for the envs with `mask` set (mw_query), into the given device tensors;
+        each output may be None.  `frame` float32 [n_envs, 18]: columns 0..17 of the next `observe`, without committing
+        the frame stack.  `pose` float64 [n_envs, K, 7] (xpos, quat w x y z) of `frames`, K ("body" | "site" | "geom",
+        name) pairs; a name a model lacks gives NaN rows.  `touching` uint8/bool [n_envs]: touching_object of the geom
+        `main_geom[slot]` names in model slot `slot` (None: 0); runs the full forward pass.  Tables are uploaded once
+        per frame list / geom list."""
+        t = self.torch
+        d_frames = None
+        if pose is not None:
+            key = ("frames", tuple(frames))
+            if key not in self._query_tables:
+                tab = np.stack([lw.query_table(frames, TARGET_ALIAS.get(s.name, ()), MOVED_SITES.get(s.name))
+                                for s, lw in zip(self.specs, self.lowered)])
+                self._query_tables[key] = t.from_numpy(tab.view(np.uint8).reshape(-1).copy()).to(self.device)
+            d_frames = self._query_tables[key]
+        d_geom = None
+        if touching is not None:
+            if len(main_geom) != len(self.specs):
+                raise ValueError(f"main_geom needs one entry per model slot ({len(self.specs)}), got {len(main_geom)}")
+            key = ("geoms", tuple(main_geom))
+            if key not in self._query_tables:
+                g = [-1 if nm is None else lw.collider(nm) for nm, lw in zip(main_geom, self.lowered)]
+                self._query_tables[key] = t.tensor(g, dtype=t.int32, device=self.device)
+            d_geom = self._query_tables[key]
+        _ck(lib().mw_query(self.h, self._p(mask), self._p(frame), self._p(d_frames), 0 if frames is None else len(frames),
+                           self._p(pose), self._p(d_geom), self._p(touching), self._stream()))
 
     FAULTS = {1: "tolerance: lower bound > upper bound (the reference raises ValueError, reward_utils.py:124)",
               2: "tolerance: margin < 0 (the reference raises ValueError, reward_utils.py:134)",

@@ -76,6 +76,11 @@ FIELDS = [
 
 DTYPE = np.dtype([(n, t, s) for n, t, s in FIELDS], align=True)
 
+# one record of an mw_query frame table (MwQueryFrame in csrc/mw_engine.cu)
+QUERY_DTYPE = np.dtype([("link", "i4"), ("flags", "i4"), ("pos", "f8", 3), ("quat", "f8", 4)])
+QF_SHIFT, QF_MISSING, QF_TARGET, QF_ADD_TARGET, QF_ADD_OBJ_INIT = 1, 2, 4, 8, 16
+MOCAP_LINK = -2      # query-table link of a frame on the mocap body (posed by the env's mocap target)
+
 # robot frames every task uses (indices are fixed; task frames follow)
 ROBOT_FRAMES = [("body", "hand"), ("body", "rightclaw"), ("body", "leftclaw"), ("body", "rightpad"),
                 ("body", "leftpad"), ("site", "rightEndEffector"), ("site", "leftEndEffector")]
@@ -108,6 +113,62 @@ class Lowered:
         self.geom_src = []       # collider index -> source geom id
         self.link_body = []      # link index -> source body id
         self.movable = None
+        self._frame_ctx = None   # (model, body pose relative to its link, link of every body, shift flag of every body)
+
+    def resolve_frame(self, kind, name):
+        """A ("body" | "site" | "geom", name) frame of the model -> (link, shift flag, pos, quat) relative to the link that
+        carries it (link -1: the world, translated at run time by the env's shift when the flag is set; MOCAP_LINK: the
+        mocap body, posed by the env's mocap target).  KeyError when the model has no such name."""
+        m, rel_pos, rel_quat, link_of_body, shifted = self._frame_ctx
+        a = m.arrays
+        if kind not in ("body", "site", "geom"):
+            raise ValueError(kind)
+        if name not in m.names[kind]:
+            raise KeyError(f"no {kind} named {name!r}")
+        i = m.names[kind].index(name)
+        if kind == "body":
+            b = i
+            fp, fq = rel_pos[b], rel_quat[b]
+        else:
+            b = a[f"{kind}_bodyid"][i]
+            fp, fq = _compose(rel_pos[b], rel_quat[b], a[f"{kind}_pos"][i], a[f"{kind}_quat"][i])
+        l = int(link_of_body[b])
+        if a["body_mocapid"][b] >= 0:      # a mocap body sits at data.mocap_pos / mocap_quat: the pose is relative to it
+            if kind == "body":
+                fp, fq = np.zeros(3), np.array([1.0, 0, 0, 0])
+            else:
+                fp, fq = a[f"{kind}_pos"][i], a[f"{kind}_quat"][i]
+            l = MOCAP_LINK
+        return l, int(l < 0 and shifted[b]), np.asarray(fp, dtype=np.float64), np.asarray(fq, dtype=np.float64)
+
+    def query_table(self, frames, target_alias=(), moved_sites=None):
+        """The mw_query frame records (QUERY_DTYPE) of a list of (kind, name) pairs; a name the model lacks gives a NaN row
+        (QF_MISSING).  `target_alias`: the frames whose position the task keeps equal to its _target_pos (QF_TARGET).
+        `moved_sites`: {site name: "target" | ("obj_init", offset)} of the sites whose model.site(name).pos the task's
+        reset_model sets to a per-episode vector; their row holds the parent body's position (+ offset) and the kernel adds
+        the env's vector (QF_ADD_TARGET / QF_ADD_OBJ_INIT)."""
+        m, rel_pos, rel_quat, link_of_body, _ = self._frame_ctx
+        t = np.zeros(len(frames), dtype=QUERY_DTYPE)
+        for k, (kind, name) in enumerate(frames):
+            try:
+                l, sh, fp, fq = self.resolve_frame(kind, name)
+            except KeyError:
+                t[k]["link"], t[k]["flags"] = -1, QF_MISSING
+                continue
+            flags = (QF_SHIFT if sh else 0) | (QF_TARGET if (kind, name) in target_alias else 0)
+            move = (moved_sites or {}).get(name) if kind == "site" else None
+            if move is not None:
+                b = m.arrays["site_bodyid"][m.names["site"].index(name)]
+                assert l == -1 and np.allclose(rel_quat[b], [1, 0, 0, 0]), "moved sites sit on static, unrotated bodies"
+                fp = rel_pos[b] + (0.0 if move == "target" else np.asarray(move[1], dtype=np.float64))
+                flags |= QF_ADD_TARGET if move == "target" else QF_ADD_OBJ_INIT
+            t[k]["link"], t[k]["pos"], t[k]["quat"], t[k]["flags"] = l, fp, fq, flags
+        return t
+
+    def collider(self, geom_name):
+        """Collider index of a source geom (the index touching_object compares contacts against), -1 when the geom takes
+        part in no contact pair or does not exist."""
+        return self.geom_names.index(geom_name) if geom_name in self.geom_names else -1
 
 
 def _compose(p1, q1, p2, q2):
@@ -348,25 +409,14 @@ def lower(m: mjcf.Model, movable: str | None, task_frames=()) -> Lowered:
     r["npair"] = len(pairs)
 
     # ---- frames
+    out._frame_ctx = (m, rel_pos, rel_quat, link_of_body, shifted)
     frames = list(ROBOT_FRAMES) + list(task_frames)
     assert len(frames) <= MAXFRAME
     for i, (kind, name) in enumerate(frames):
-        if kind == "body":
-            b = m.names["body"].index(name)
-            fp, fq = rel_pos[b], rel_quat[b]
-        elif kind == "geom":
-            g = m.names["geom"].index(name)
-            b = a["geom_bodyid"][g]
-            fp, fq = _compose(rel_pos[b], rel_quat[b], a["geom_pos"][g], a["geom_quat"][g])
-        elif kind == "site":
-            s = m.names["site"].index(name)
-            b = a["site_bodyid"][s]
-            fp, fq = _compose(rel_pos[b], rel_quat[b], a["site_pos"][s], a["site_quat"][s])
-        else:
-            raise ValueError(kind)
-        l = link_of_body[b]
+        l, sh, fp, fq = out.resolve_frame(kind, name)
+        assert l != MOCAP_LINK, "the step kernels read no frame on the mocap body"
         r["frame_link"][i] = l
-        r["frame_shift"][i] = int(l < 0 and shifted[b])
+        r["frame_shift"][i] = sh
         r["frame_pos"][i] = fp
         r["frame_quat"][i] = fq
         out.frame_names.append((kind, name))

@@ -21,11 +21,11 @@ from __future__ import annotations
 
 import numpy as np
 
-from . import _gym
+from . import _gym, modelzoo
 from .benchmarks import REFERENCE_CLASS, Task
 from .engine import INFO_KEYS, MAXDOF, MAXNQ, Engine, lowered
-from .tasks import TASKS
-from .vector_env import MAX_PATH_LENGTH, MetaWorldVecEnv
+from .tasks import ACHIEVED_GOAL, MAIN_OBJECT, TARGET_ALIAS, TASKS
+from .vector_env import _TWO_OBJECTS, MAX_PATH_LENGTH, STATE_CALLS, MetaWorldVecEnv
 
 _HAND_LOW = np.array([-0.525, 0.348, -0.0525])     # SawyerXYZEnv._HAND_SPACE (sawyer_xyz_env.py:146-150)
 _HAND_HIGH = np.array([+0.525, 1.025, 0.7])
@@ -61,7 +61,11 @@ class SawyerXYZEnvB200:
         self.engine.set_envs([0])
         # no wrapper here: the horizon check is SawyerXYZEnv's own (max_path_length), success never terminates
         self.engine.set_options(MAX_PATH_LENGTH, False, 0)
+        # autoreset off (the horizon is SawyerXYZEnv's own): at truncation the env keeps its terminal state, which the
+        # state getters read, until reset().  This also applies to an engine passed in through `engine=`.
+        self.engine.set_autoreset_mode("Disabled")
         self.curr_path_length = 0
+        self._goal_site_written = False
         self._partially_observable = True            # until set_task (sawyer_xyz_env.py:208)
         self._set_task_called = False
         self._last_rand_vec = None
@@ -129,6 +133,7 @@ class SawyerXYZEnvB200:
         self.d_sid[0] = self._snap_id
         self.engine.reset(self.d_sid, self.d_obs)
         self._did_reset = True
+        self._goal_site_written = self.env_name == "shelf-place-v3"
         return self.d_obs[0].cpu().numpy().astype(np.float64), {}
 
     @_assert_task_is_set
@@ -142,10 +147,11 @@ class SawyerXYZEnvB200:
         self.d_act[0] = self.torch.as_tensor(np.asarray(action, dtype=np.float32))
         self.engine.step(self.d_act, self.d_obs, self.d_rew, self.d_term, self.d_trunc, self.d_info, self.d_fobs, self.d_finfo, self.d_sid)
         self.curr_path_length += 1
+        self._goal_site_written = False
         rec = self.d_info[0].cpu().numpy()
         truncate = self.curr_path_length == self.max_path_length
-        # at the horizon the kernel has already restarted the episode (SAME_STEP): the terminal observation is in final_obs
-        obs = (self.d_fobs if truncate else self.d_obs)[0].cpu().numpy().astype(np.float64)
+        # autoreset is off: at the horizon the env keeps its terminal state (the state getters read it) until reset()
+        obs = self.d_obs[0].cpu().numpy().astype(np.float64)
         self._last_stable_obs = obs
         info = {k: float(rec[i]) for i, k in enumerate(INFO_KEYS)}
         return obs, float(rec[7]), False, truncate, info
@@ -174,6 +180,8 @@ class SawyerXYZEnvB200:
 
     @property
     def _target_pos(self):
+        if self.env_name in TARGET_ALIAS:      # a view of data.site("goal").xpos in the reference: live
+            return self._query(TARGET_ALIAS[self.env_name])[1][0, :3].copy()
         return self._state()["target"].astype(np.float64)
 
     @property
@@ -200,6 +208,7 @@ class SawyerXYZEnvB200:
         q = np.zeros((1, MAXNQ)); q[0, :nq] = qpos
         v = np.zeros((1, MAXDOF)); v[0, :nv] = qvel
         self.engine.set_physics(t.ones(1, dtype=t.bool, device=dev), t.from_numpy(q).to(dev), t.from_numpy(v).to(dev))
+        self._goal_site_written = False      # MujocoEnv.set_state runs mj_forward
 
     def set_env_state(self, state):
         """SawyerMocapBase.set_env_state((qpos, qvel)) (sawyer_xyz_env.py:97-107)."""
@@ -215,6 +224,100 @@ class SawyerXYZEnvB200:
         out = t.zeros(1, 39, device=dev)
         self.engine.observe(t.ones(1, dtype=t.bool, device=dev), out)
         return out[0].cpu().numpy().astype(np.float64)
+
+    # ---- state getters (sawyer_xyz_env.py:67-85, 363-473, 529-535; MujocoEnv.get_body_com), computed by mw_query
+    def _query(self, frames=(), touching_geom=None):
+        if not self._did_reset:
+            raise RuntimeError("reset() must be called before reading the state (the device state is created by reset)")
+        t, dev = self.torch, self.engine.device
+        frame = t.zeros(1, 18, device=dev)
+        pose = t.zeros(1, len(frames), 7, dtype=t.float64, device=dev) if frames else None
+        touch = t.zeros(1, dtype=t.bool, device=dev) if touching_geom is not None else None
+        self.engine.query(t.ones(1, dtype=t.bool, device=dev), frame=frame, pose=pose, frames=list(frames) or None,
+                          touching=touch, main_geom=[touching_geom])
+        return frame[0].cpu().numpy(), None if pose is None else pose[0].cpu().numpy(), None if touch is None else bool(touch[0])
+
+    def _check_name(self, kind, name):
+        names = modelzoo.full_model(self.spec_.xml).names[kind]
+        if name not in names:
+            raise KeyError(f"Invalid name '{name}'. Valid names: {names}")
+
+    def get_endeff_pos(self):
+        """data.body("hand").xpos: the float32 value the observation carries (obs[:3] before clipping), as float64."""
+        return self._query()[0][:3].astype(np.float64)
+
+    @property
+    def tcp_center(self):
+        p = self._query((("site", "rightEndEffector"), ("site", "leftEndEffector")))[1]
+        return (p[0, :3] + p[1, :3]) / 2.0
+
+    def _get_pos_objects(self):
+        f = self._query()[0]
+        return np.concatenate([f[4:7], f[11:14]] if self.env_name in _TWO_OBJECTS else [f[4:7]]).astype(np.float64)
+
+    def _get_quat_objects(self):
+        f = self._query()[0]
+        return np.concatenate([f[7:11], f[14:18]] if self.env_name in _TWO_OBJECTS else [f[7:11]]).astype(np.float64)
+
+    def _get_pos_goal(self):
+        return self._target_pos
+
+    def _get_obs_dict(self):
+        obs = self._get_obs()
+        return dict(state_observation=obs, state_desired_goal=self._get_pos_goal(), state_achieved_goal=self._achieved_goal(obs))
+
+    def _achieved_goal(self, obs):
+        how = ACHIEVED_GOAL.get(self.env_name)
+        if how is None:
+            return obs[3:-3]
+        if how == "objects":
+            return self._get_pos_objects()
+        kind, name, offset = how
+        p = self._query(((kind, name),))[1][0, :3].copy()
+        return p if offset is None else p + np.asarray(offset)
+
+    def _get_site_pos(self, site_name):
+        self._check_name("site", site_name)
+        if site_name == "goal" and self._goal_site_written:
+            return self._target_pos        # reset_model's _set_pos_site("goal", ...) holds until the next forward pass
+        return self._query((("site", site_name),))[1][0, :3].copy()
+
+    def get_body_com(self, body_name):
+        self._check_name("body", body_name)
+        return self._query((("body", body_name),))[1][0, :3].copy()
+
+    def _get_id_main_object(self):
+        spec = MAIN_OBJECT[self.env_name]
+        if spec is None:
+            return None
+        geom, lookup = spec
+        if lookup == "name2id":
+            raise AttributeError("'MjModel' object has no attribute 'geom_name2id'")
+        self._check_name("geom", geom)
+        return modelzoo.full_model(self.spec_.xml).names["geom"].index(geom)
+
+    def touching_object(self, object_geom_id):
+        names = modelzoo.full_model(self.spec_.xml).names["geom"]
+        if object_geom_id is None or not 0 <= int(object_geom_id) < len(names):
+            return False                   # no contact involves such a geom
+        return self._query(touching_geom=names[int(object_geom_id)])[2]
+
+    @property
+    def touching_main_object(self):
+        return self.touching_object(self._get_id_main_object())
+
+    @property
+    def init_tcp(self):
+        return self._state()["init_tcp"].astype(np.float64)
+
+    # sawyer_xyz_env.py:236-237 keeps get_body_com("leftpad" / "rightpad"), a view of data.body(..).xpos: the live pad
+    @property
+    def init_left_pad(self):
+        return self.get_body_com("leftpad")
+
+    @property
+    def init_right_pad(self):
+        return self.get_body_com("rightpad")
 
     def close(self):
         if self._own_engine and self.engine is not None:
@@ -263,7 +366,8 @@ class MetaWorldSingleEnv:
 
     # the attribute / method names reached through env.unwrapped / get_wrapper_attr in the reference
     def __getattr__(self, name):
-        if name in ("toggle_terminate_on_success", "toggle_sample_tasks_on_reset", "sample_tasks", "get_checkpoint", "load_checkpoint"):
+        if name in ("toggle_terminate_on_success", "toggle_sample_tasks_on_reset", "sample_tasks", "get_checkpoint",
+                    "load_checkpoint") + STATE_CALLS:
             def call(*a, **k):
                 out = self.vec.call(name, *a, **k)
                 return out[0] if isinstance(out, tuple) and len(out) == 1 else out

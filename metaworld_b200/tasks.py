@@ -210,6 +210,44 @@ _SPECS = [
 
 TASKS = {t.name: t for t in _SPECS}
 TASK_IDS = {t.name: t.task_id for t in _SPECS}
+
+# What each reference class's `_get_id_main_object()` does (SawyerXYZEnv default: data.geom("objGeom").id,
+# sawyer_xyz_env.py:442-443, and the per-task overrides): None = returns None; otherwise (geom name, lookup), where
+# lookup "name2id" is `model.geom_name2id(...)`, which MuJoCo's Python bindings do not have (the reference raises
+# AttributeError), and "geom" is `data.geom(name).id` / `model.geom(name).id` (KeyError when the model has no such geom).
+_NAME2ID = ("drawer-open-v3", "button-press-topdown-v3", "pick-out-of-hole-v3", "button-press-v3", "button-press-wall-v3",
+            "button-press-topdown-wall-v3", "assembly-v3", "disassemble-v3", "basketball-v3", "bin-picking-v3",
+            "box-close-v3", "hammer-v3", "lever-pull-v3")
+_MAIN_GEOM = {"button-press-topdown-v3": "btnGeom", "button-press-v3": "btnGeom", "button-press-wall-v3": "btnGeom",
+              "button-press-topdown-wall-v3": "btnGeom", "coffee-pull-v3": "mug", "coffee-push-v3": "mug",
+              "assembly-v3": "WrenchHandle", "disassemble-v3": "WrenchHandle", "box-close-v3": "BoxHandleGeom",
+              "hammer-v3": "HammerHandle"}
+# frames whose position a task keeps equal to its _target_pos after every forward pass (csrc/mw_tasks_gen.cuh
+# task_live_update): basketball's _target_pos aliases data.site("goal").xpos
+TARGET_ALIAS = {"basketball-v3": (("site", "goal"),)}
+# sites whose model.site(name).pos a task's reset_model sets to a per-episode vector (e.g. sawyer_reach_v3.py:134): the
+# site then sits at (its body's position) + that vector.  "target": _target_pos; ("obj_init", offset): obj_init_pos +
+# offset (sawyer_disassemble_peg_v3.py:128-131).  Basketball's goal is live instead (TARGET_ALIAS); shelf-place writes the
+# site's xpos only (_set_pos_site), which the next forward pass undoes.
+_GOAL_IS_TARGET = ("reach-v3", "push-v3", "pick-place-v3", "door-open-v3", "drawer-open-v3", "drawer-close-v3",
+                   "peg-insert-side-v3", "window-open-v3", "window-close-v3", "reach-wall-v3", "push-wall-v3",
+                   "pick-place-wall-v3", "push-back-v3", "sweep-v3", "sweep-into-v3", "hand-insert-v3", "pick-out-of-hole-v3",
+                   "dial-turn-v3", "door-close-v3", "box-close-v3", "lever-pull-v3", "peg-unplug-side-v3", "plate-slide-v3",
+                   "plate-slide-side-v3", "plate-slide-back-v3", "plate-slide-back-side-v3", "soccer-v3", "stick-push-v3",
+                   "stick-pull-v3")
+MOVED_SITES = {**{t: {"goal": "target"} for t in _GOAL_IS_TARGET},
+               "coffee-pull-v3": {"mug_goal": "target"}, "coffee-push-v3": {"mug_goal": "target"},
+               "faucet-open-v3": {"goal_open": ("obj_init", (0.175, 0.0, 0.125))},      # sawyer_faucet_open_v3.py:111-114
+               "faucet-close-v3": {"goal_close": ("obj_init", (-0.175, 0.0, 0.125))},   # sawyer_faucet_close_v3.py
+               "assembly-v3": {"pegTop": "target"}, "disassemble-v3": {"pegTop": ("obj_init", (0.0, 0.0, 0.08))}}
+# tasks whose _get_obs_dict() overrides state_achieved_goal (default: obs[3:-3]): a (kind, name, offset) frame position,
+# or "objects" = _get_pos_objects() (sawyer_assembly_peg_v3.py:110-113, sawyer_disassemble_peg_v3.py:111-114,
+# sawyer_stick_push_v3.py:126-131, sawyer_stick_pull_v3.py:131-134, sawyer_plate_slide_back_side_v3.py:114-119)
+ACHIEVED_GOAL = {"assembly-v3": ("body", "RoundNut", None), "disassemble-v3": ("body", "RoundNut", None),
+                 "stick-push-v3": ("site", "insertion", (0.0, 0.09, 0.0)), "stick-pull-v3": ("site", "insertion", None),
+                 "plate-slide-back-side-v3": "objects"}
+MAIN_OBJECT = {t.name: None if t.name in ("door-lock-v3", "door-unlock-v3", "coffee-button-v3")
+               else (_MAIN_GEOM.get(t.name, "objGeom"), "name2id" if t.name in _NAME2ID else "geom") for t in _SPECS}
 assert sorted(TASK_IDS.values()) == list(range(len(_SPECS)))
 
 

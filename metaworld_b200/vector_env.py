@@ -27,12 +27,29 @@ import base64
 
 import numpy as np
 
-from . import _gym
+from . import _gym, modelzoo
 from .benchmarks import Task, reference_env_id
 from .engine import ENVSTATE_DTYPE, INFO_KEYS, MAXDOF, MAXNQ, Engine, expert_actions, lowered
-from .tasks import TASK_IDS, TASKS
+from .tasks import ACHIEVED_GOAL, MAIN_OBJECT, TARGET_ALIAS, TASK_IDS, TASKS
 
 MAX_PATH_LENGTH = 500     # SawyerXYZEnv.max_path_length (sawyer_xyz_env.py:152): truncates whatever TimeLimit says
+_TWO_OBJECTS = ("hammer-v3", "stick-push-v3", "stick-pull-v3")   # _get_pos_objects has 6 elements, _get_quat_objects 8
+# the reference getters that `call` / `get_attr` reach on every sub-env (SyncVectorEnv forwards them)
+STATE_CALLS = ("get_endeff_pos", "_get_pos_objects", "_get_quat_objects", "_get_pos_goal", "_get_obs_dict", "_get_site_pos",
+               "get_body_com", "touching_object", "_get_id_main_object")
+STATE_ATTRS = ("tcp_center", "touching_main_object", "_target_pos", "obj_init_pos", "init_tcp", "init_left_pad",
+               "init_right_pad", "hand_init_pos")
+
+
+def _quat2mat(q):
+    """[..., 4] unit quaternions (w, x, y, z) -> [..., 3, 3] rotation matrices (MuJoCo's mju_quat2Mat), on the device."""
+    import torch
+
+    w, x, y, z = q.unbind(-1)
+    r = [1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y),
+         2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x),
+         2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)]
+    return torch.stack(r, -1).view(q.shape[:-1] + (3, 3))
 
 
 def _serialize_task(task: Task) -> dict:          # metaworld/wrappers.py:35-39
@@ -732,6 +749,163 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self.engine.observe(self._device_mask(env_mask), self.d_env_obs)
         return self.d_env_obs.cpu().numpy().astype(np.float64)
 
+    # ------------------------------------------------------------------ state accessors (SawyerXYZEnv / MujocoEnv getters)
+    def query_torch(self, env_mask=None, bodies=(), sites=(), geoms=(), touching=False):
+        """Read-only accessors of every env's current state (envs with `env_mask` set; bool tensor [num_envs], None =
+        all), as a dict of new device tensors, without host synchronisation and without changing any state:
+
+        * ``frame``: float32 [num_envs, 18], columns 0..17 of the next `observe_torch` (hand, gripper distance, the 14
+          object slots), unclipped; the frame stack is not advanced.
+        * ``body_xpos`` / ``body_xquat`` (float64 [num_envs, len(bodies), 3] / [.., 4], w x y z), ``site_xpos`` /
+          ``site_xmat`` ([.., 3] / [.., 3, 3]) and ``geom_xpos`` / ``geom_xmat``: MuJoCo's data.body / site / geom(name)
+          poses; a name an env's model lacks gives NaN.
+        * ``touching`` (when `touching`): bool [num_envs], the reference's ``touching_main_object`` for the geom its
+          ``_get_id_main_object`` names, False where that returns None.  Runs the full forward pass (contact forces).
+
+        Rows of the other envs are zero (their ``*_xmat`` rows: the identity, the matrix of a zero quaternion)."""
+        self._check_started("query_torch")
+        t = self.torch
+        mask = self._torch_mask(env_mask)
+        groups = (("body", bodies), ("site", sites), ("geom", geoms))
+        for kind, names in groups:
+            if isinstance(names, str) or not all(isinstance(n, str) for n in names):
+                raise ValueError(f"query_torch: {kind}s must be a sequence of {kind} names")
+        frames = [(kind, n) for kind, names in groups for n in names]
+        N = self.num_envs
+        out = {"frame": t.zeros(N, 18, dtype=t.float32, device=self.device)}
+        pose = t.zeros(N, len(frames), 7, dtype=t.float64, device=self.device) if frames else None
+        touch = t.zeros(N, dtype=t.bool, device=self.device) if touching else None
+        main = [None if MAIN_OBJECT[n] is None else MAIN_OBJECT[n][0] for n in dict.fromkeys(self.env_names)]   # per model slot
+        self.engine.query(mask, frame=out["frame"], pose=pose, frames=frames or None, touching=touch, main_geom=main)
+        k = 0
+        for kind, names in groups:
+            p = pose[:, k:k + len(names)] if frames else t.zeros(N, 0, 7, dtype=t.float64, device=self.device)
+            k += len(names)
+            out[f"{kind}_xpos"] = p[..., :3]
+            if kind == "body":
+                out["body_xquat"] = p[..., 3:]
+            else:
+                out[f"{kind}_xmat"] = _quat2mat(p[..., 3:])
+        if touching:
+            out["touching"] = touch
+        return out
+
+    def _query_host(self, **kw):
+        """`query_torch` for every env, copied to numpy (the host-side getters of `call` / `get_attr`)."""
+        return {k: v.cpu().numpy() for k, v in self.query_torch(**kw).items()}
+
+    def _obs_slots(self, e, frame, what):
+        """The reference's _get_pos_objects / _get_quat_objects of env e: the observation's object slots (3 / 6 positions,
+        4 / 8 quaternions) as float64."""
+        two = self.sub[e].task_name in _TWO_OBJECTS
+        if what == "pos":
+            return np.concatenate([frame[4:7], frame[11:14]] if two else [frame[4:7]]).astype(np.float64)
+        return np.concatenate([frame[7:11], frame[14:18]] if two else [frame[7:11]]).astype(np.float64)
+
+    def _main_object_id(self, e):
+        """_get_id_main_object() of env e: the source geom id, None, or the reference's exception."""
+        spec = MAIN_OBJECT[self.sub[e].task_name]
+        if spec is None:
+            return None
+        geom, lookup = spec
+        if lookup == "name2id":
+            raise AttributeError("'MjModel' object has no attribute 'geom_name2id'")
+        names = modelzoo.full_model(TASKS[self.sub[e].task_name].xml).names["geom"]
+        if geom not in names:
+            raise KeyError(f"Invalid name '{geom}'. Valid names: {names}")
+        return names.index(geom)
+
+    def _call_getter(self, name, args):
+        """`call` of the reference's SawyerXYZEnv / MujocoEnv getters (metaworld/sawyer_xyz_env.py:67-85, 363-473,
+        529-535): one value per sub-env, computed on the device by `query_torch`."""
+        self._check_started(name)
+        N = self.num_envs
+        if name in ("get_endeff_pos", "_get_pos_objects", "_get_quat_objects"):
+            fr = self._query_host()["frame"]
+            if name == "get_endeff_pos":
+                return tuple(fr[e, :3].astype(np.float64) for e in range(N))
+            return tuple(self._obs_slots(e, fr[e], "pos" if name == "_get_pos_objects" else "quat") for e in range(N))
+        if name == "_get_pos_goal":
+            return self.get_attr("_target_pos")
+        if name == "_get_obs_dict":
+            obs = self.observe()
+            goal = self.get_attr("_target_pos")
+            ach = [obs[e, 3:36].copy() for e in range(N)]
+            for e in range(N):
+                how = ACHIEVED_GOAL.get(self.sub[e].task_name)
+                if how == "objects":
+                    ach[e] = self._call_getter("_get_pos_objects", ())[e]
+                elif how is not None:
+                    kind, nm, offset = how
+                    p = self._query_host(**{"sites" if kind == "site" else "bodies": (nm,)})[f"{kind}_xpos"][e, 0].copy()
+                    ach[e] = p if offset is None else p + np.asarray(offset)
+            return tuple(dict(state_observation=obs[e, :39].copy(), state_desired_goal=goal[e], state_achieved_goal=ach[e])
+                         for e in range(N))
+        if name in ("_get_site_pos", "get_body_com"):
+            (nm,) = args
+            kind = "site" if name == "_get_site_pos" else "body"
+            self._check_names(kind, nm)
+            q = self._query_host(**{"sites" if kind == "site" else "bodies": (nm,)})
+            return tuple(q[f"{kind}_xpos"][e, 0].copy() for e in range(N))
+        if name == "_get_id_main_object":
+            return tuple(self._main_object_id(e) for e in range(N))
+        if name == "touching_object":
+            (gid,) = args
+            return self._touching([self._geom_name(e, gid) for e in range(N)])
+        raise AttributeError(name)
+
+    def _check_names(self, kind, name):
+        for s in {s.task_name for s in self.sub}:
+            names = modelzoo.full_model(TASKS[s].xml).names[kind]
+            if name not in names:
+                raise KeyError(f"Invalid name '{name}'. Valid names: {names}")
+
+    def _geom_name(self, e, gid):
+        names = modelzoo.full_model(TASKS[self.sub[e].task_name].xml).names["geom"]
+        return names[gid] if gid is not None and 0 <= int(gid) < len(names) else None
+
+    def _touching(self, geom_per_env):
+        """touching_object of one geom name per env (None: False), on the device."""
+        t = self.torch
+        out = np.zeros(self.num_envs, dtype=bool)
+        for g in set(geom_per_env):
+            if g is None:
+                continue
+            rows = np.array([x == g for x in geom_per_env])
+            touch = t.zeros(self.num_envs, dtype=t.bool, device=self.device)
+            self.engine.query(t.from_numpy(rows).to(self.device), touching=touch, main_geom=[g] * len(set(self.env_names)))
+            out |= touch.cpu().numpy() & rows
+        return tuple(bool(x) for x in out)
+
+    def _attr_getter(self, name):
+        """`get_attr` of the reference's state attributes, one value per sub-env."""
+        N = self.num_envs
+        if name in ("_target_pos", "obj_init_pos", "init_tcp"):
+            self._check_started(name)
+            st = self.engine.get_state()
+            key = {"_target_pos": "target", "obj_init_pos": "obj_init", "init_tcp": "init_tcp"}[name]
+            if name == "_target_pos":      # basketball's goal is live (data.site("goal").xpos): refresh it like the kernels do
+                fr = self._query_host(sites=("goal",))["site_xpos"][:, 0]
+                return tuple(fr[e].copy() if self.sub[e].task_name in TARGET_ALIAS else st[key][e].astype(np.float64)
+                             for e in range(N))
+            return tuple(st[key][e].astype(np.float64) for e in range(N))
+        if name == "tcp_center":
+            self._check_started(name)
+            x = self._query_host(sites=("rightEndEffector", "leftEndEffector"))["site_xpos"]
+            return tuple((x[e, 0] + x[e, 1]) / 2.0 for e in range(N))
+        if name == "touching_main_object":
+            self._check_started(name)
+            for e in range(N):
+                self._main_object_id(e)           # the reference's exceptions
+            return tuple(bool(x) for x in self._query_host(touching=True)["touching"])
+        if name in ("init_left_pad", "init_right_pad"):      # views of data.body(..).xpos in the reference: the live pad
+            self._check_started(name)
+            x = self._query_host(bodies=("leftpad" if name == "init_left_pad" else "rightpad",))["body_xpos"]
+            return tuple(x[e, 0].copy() for e in range(N))
+        if name == "hand_init_pos":
+            return tuple(np.array(TASKS[s.task_name].hand_init_pos, dtype=np.float64) for s in self.sub)
+        raise AttributeError(name)
+
     # ------------------------------------------------------------------ scripted experts (metaworld.policies)
     def expert_actions_torch(self, obs=None):
         """Every env's scripted expert action (metaworld_b200.policies: its task's policy in ENV_POLICY_MAP), as a new
@@ -806,6 +980,8 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             return tuple(s.sample_tasks_on_reset for s in self.sub)
         if name == "env_id":
             return tuple(s.env_id for s in self.sub)
+        if name in STATE_ATTRS:
+            return self._attr_getter(name)
         raise AttributeError(name)
 
     def set_attr(self, name, values):
@@ -860,6 +1036,8 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         if name == "_get_obs":                  # SawyerXYZEnv._get_obs(): the base env's 39 columns
             obs = self.observe()
             return tuple(obs[e, :39].copy() for e in range(self.num_envs))
+        if name in STATE_CALLS:
+            return self._call_getter(name, args)
         return self.get_attr(name)
 
     # ------------------------------------------------------------------ checkpoint (metaworld/wrappers.py:125-142,190-204,275-322)
