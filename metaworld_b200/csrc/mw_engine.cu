@@ -70,6 +70,7 @@ struct WarpShared {
   float obs[40]; float info[8];
 };
 static size_t smem_bytes() { return sizeof(BlockShared) + WARPS_PER_BLOCK * sizeof(WarpShared) + 16; }
+extern __shared__ __align__(16) unsigned char smem[];   // the CTA kernels' BlockShared, then one WarpShared per warp
 
 DEV unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 // TMA bulk copy global -> shared with mbarrier completion (SASS: UBLKCP / SYNCS)
@@ -127,6 +128,63 @@ DEV void store_env(WarpShared* ws, MwEnvState* dst, int lane) {
   ((float4*)dst)[lane] = ((const float4*)&ws->es)[lane];
 }
 
+// ---------------------------------------------------------------- CTA kernel prologue
+// The CTA table (make_blocks): work item b runs the count[b] envs perm[start[b]], perm[start[b] + 1], ... (k_snapshot:
+// snapshot items) of model slot model[b], one warp each.
+struct BlockTable { const int *model, *start, *count, *perm; };
+
+// One warp's place in a CTA kernel (cta_enter)
+struct CtaWarp {
+  BlockShared* bs; WarpShared* ws; WarpScratch* w; const MwModel* m;
+  int mi, lane, env;                                   // model slot, lane, this warp's env (k_snapshot: snapshot item)
+};
+
+// Entry of every CTA kernel for work item `blk` of `bt`: stages the item's model, then places each warp on its env, wires
+// its global scratch slots and joins it to the CTA's convex-pair queue (`hints`: with the env's row of the separating-axis
+// hint table; k_step only).  Barriers: every thread of the CTA takes part in the two __syncthreads of stage_model; a warp
+// past count[blk] then returns false and its kernel returns before join_cta, so the CTA's phase barriers count only the
+// count[blk] warps that have an env.
+DEV bool cta_enter(const EngineDev& e, const BlockTable& bt, int blk, CtaWarp& cw, bool hints = false) {
+  cw.bs = (BlockShared*)smem;
+  WarpShared* wsa = (WarpShared*)(smem + sizeof(BlockShared));
+  cw.mi = bt.model[blk];
+  stage_model(cw.bs, e.models + (size_t)cw.mi * e.model_stride, (unsigned)sizeof(cw.bs->model), e.taskconsts + cw.mi);
+  const int warp = threadIdx.x >> 5, live = bt.count[blk];
+  cw.lane = threadIdx.x & 31;
+  if (warp >= live) return false;
+  cw.env = bt.perm[bt.start[blk] + warp];
+  cw.ws = wsa + warp;
+  cw.ws->w.epa = e.epa + scratch_slot(e, warp);
+  cw.ws->w.sp = e.spill + scratch_slot(e, warp);
+  cw.w = &cw.ws->w;
+  join_cta(cw.bs, wsa, cw.w, warp, live, hints ? e.sep_hint + (size_t)cw.env * MW_NCONV : nullptr);
+  cw.m = (const MwModel*)cw.bs->model;
+  return true;
+}
+
+// load_env, then the per-step scratch reset: profile counters and fault bits zeroed, phase timers on or off (`prof_on`)
+DEV void enter_env(const EngineDev& e, const CtaWarp& cw, int prof_on) {
+  load_env(cw.ws, e.state + cw.env, cw.lane);
+  if (cw.lane < 16) cw.w->prof[cw.lane] = 0;
+  if (cw.lane == 0) { cw.w->fault = 0; cw.w->prof_on = prof_on; }
+  SYNCW();
+}
+
+DEV TaskCtx task_ctx(const EngineDev& e, const CtaWarp& cw, const real* action) {
+  TaskCtx c; c.m = cw.m; c.tc = &cw.bs->tc; c.w = cw.w; c.s = &cw.ws->es; c.action = action; c.meshvert = e.meshverts[cw.mi];
+  return c;
+}
+
+// Whether any env of work item `blk` has mask[env] set.  The kernels that act on masked envs only (k_observe, k_query)
+// return at once when it is false: every thread of the CTA reads the same mask bytes, so the whole CTA leaves before its
+// first barrier.  In a CTA that stays, the unmasked warps run the same pass as the masked ones, so they meet every
+// barrier, and skip only the writes after the pass.
+DEV bool cta_has_masked(const BlockTable& bt, int blk, const unsigned char* __restrict__ mask) {
+  bool any = false;
+  for (int k = 0; k < bt.count[blk]; k++) any = any || mask[bt.perm[bt.start[blk] + k]];
+  return any;
+}
+
 // observation assembly (sawyer_xyz_env.py:475-527 + clip :623-628); lane 0
 DEV void make_obs(const TaskCtx& c, float* obs, bool clip = true) {   // reset() returns the observation unclipped (:664-682)
   real cur[18];
@@ -162,39 +220,25 @@ DEV int sample_snapshot(const EngineDev& e, int env, float episode) {
 // so that the default path carries none of the code of the other modes (the kernel is bound by instruction fetch)
 template <bool DEFERRED>
 __global__ void __launch_bounds__(BLOCK_THREADS, 1)
-k_step(EngineDev e, const int* __restrict__ block_order, const int* __restrict__ block_model, const int* __restrict__ block_start, const int* __restrict__ block_count,
-       const int* __restrict__ perm, const float* __restrict__ actions, float* __restrict__ obs_out, int obs_stride,
+k_step(EngineDev e, const int* __restrict__ block_order, BlockTable bt, const float* __restrict__ actions, float* __restrict__ obs_out, int obs_stride,
        float* __restrict__ reward, unsigned char* __restrict__ terminated, unsigned char* __restrict__ truncated,
        float* __restrict__ info_out, int info_stride, float* __restrict__ final_obs, float* __restrict__ final_info, const int* __restrict__ next_snapshot,
        const int* __restrict__ block_live) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  BlockShared* bs = (BlockShared*)smem;
-  WarpShared* wsa = (WarpShared*)(smem + sizeof(BlockShared));
   const int blk = block_order[blockIdx.x];             // launch slot -> CTA work item (costliest first, see k_order_*)
   if (block_live && !block_live[blk]) return;          // the other decomposition of this model's head is running (k_order_blocks)
-  const int mi = block_model[blk];
-  stage_model(bs, e.models + (size_t)mi * e.model_stride, (unsigned)sizeof(bs->model), e.taskconsts + mi);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp >= block_count[blk]) return;
-  const int env = perm[block_start[blk] + warp];
-  WarpShared* ws = wsa + warp;
-  ws->w.epa = e.epa + scratch_slot(e, warp);
-  ws->w.sp = e.spill + scratch_slot(e, warp);
-  WarpScratch* w = &ws->w;
-  join_cta(bs, wsa, w, warp, block_count[blk], e.sep_hint + (size_t)env * MW_NCONV);
-  const MwModel* m = (const MwModel*)bs->model;
-  load_env(ws, e.state + env, lane);
+  CtaWarp cw;
+  if (!cta_enter(e, bt, blk, cw, /*hints=*/true)) return;
+  BlockShared* bs = cw.bs; WarpShared* ws = cw.ws; WarpScratch* w = cw.w; const MwModel* m = cw.m;
+  const int mi = cw.mi, lane = cw.lane, env = cw.env;
+  enter_env(e, cw, e.prof != nullptr);
   // NEXT_STEP / DISABLED: an env whose episode ended in the previous call still runs its physics below, so that its warp
   // takes part in the CTA's phase barriers, and the result is discarded in the tail (restart, or nothing at all)
   const bool ended = DEFERRED && ws->es.ended != 0.f;
-  if (lane < 16) w->prof[lane] = 0;
-  if (lane == 0) { w->fault = 0; w->prof_on = e.prof != nullptr; }
-  SYNCW();
   const long long t_begin = MW_CLK(w);
   const long long t_cta = e.env_cycles ? mw_clock() : 0ll;
   real act[4];
   for (int i = 0; i < 4; i++) act[i] = fmin(fmax((real)actions[4 * env + i], (real)-1), (real)1);
-  TaskCtx c; c.m = m; c.tc = &bs->tc; c.w = w; c.s = &ws->es; c.action = act; c.meshvert = e.meshverts[mi];
+  TaskCtx c = task_ctx(e, cw, act);
   // set_xyz_action (sawyer_xyz_env.py:320-336) + ctrl = [a3, -a3] (:595)
   if (lane < 3) w->mocap_pos[lane] = fmin(fmax(w->mocap_pos[lane] + act[lane] * (real)0.01, (real)bs->tc.mocap_lo[lane]), (real)bs->tc.mocap_hi[lane]);
   if (lane == 0) { w->ctrl[0] = (real)actions[4 * env + 3]; w->ctrl[1] = -(real)actions[4 * env + 3]; }
@@ -305,26 +349,15 @@ k_step(EngineDev e, const int* __restrict__ block_order, const int* __restrict__
 
 // builds episode-start snapshots: exact reset() sequence of the reference (reset_model, mj_resetData, reset_model)
 __global__ void __launch_bounds__(BLOCK_THREADS, 1)
-k_snapshot(EngineDev e, const int* __restrict__ block_model, const int* __restrict__ block_start, const int* __restrict__ block_count,
-           const int* __restrict__ perm, const double* __restrict__ rand_vec, const double* __restrict__ rand_vec_pass1, const unsigned char* __restrict__ partial, int snap_base) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  BlockShared* bs = (BlockShared*)smem;
-  WarpShared* wsa = (WarpShared*)(smem + sizeof(BlockShared));
-  const int mi = block_model[blockIdx.x];
-  stage_model(bs, e.models + (size_t)mi * e.model_stride, (unsigned)sizeof(bs->model), e.taskconsts + mi);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp >= block_count[blockIdx.x]) return;
-  const int item = perm[block_start[blockIdx.x] + warp];
-  WarpShared* ws = wsa + warp;
-  ws->w.epa = e.epa + scratch_slot(e, warp);
-  ws->w.sp = e.spill + scratch_slot(e, warp);
-  WarpScratch* w = &ws->w;
-  join_cta(bs, wsa, w, warp, block_count[blockIdx.x]);
-  const MwModel* m = (const MwModel*)bs->model;
+k_snapshot(EngineDev e, BlockTable bt, const double* __restrict__ rand_vec, const double* __restrict__ rand_vec_pass1, const unsigned char* __restrict__ partial, int snap_base) {
+  CtaWarp cw;
+  if (!cta_enter(e, bt, blockIdx.x, cw)) return;
+  BlockShared* bs = cw.bs; WarpShared* ws = cw.ws; WarpScratch* w = cw.w; const MwModel* m = cw.m;
+  const int lane = cw.lane, item = cw.env;
   const double* rv2 = rand_vec + 6 * item;
   const double* rv1 = rand_vec_pass1 ? rand_vec_pass1 + 6 * item : rv2;   // an unfrozen rand_vec draws once per reset_model pass
   real act[4] = {0, 0, 0, 0};
-  TaskCtx c; c.m = m; c.tc = &bs->tc; c.w = w; c.s = &ws->es; c.action = act; c.meshvert = e.meshverts[mi];
+  TaskCtx c = task_ctx(e, cw, act);
   for (int i = lane; i < 128; i += 32) ((float*)&ws->es)[i] = 0.f;
   if (lane < 3) w->shift[lane] = 0;
   SYNCW();
@@ -395,21 +428,11 @@ __global__ void k_reset_masked(EngineDev e, const unsigned char* __restrict__ ma
 }
 
 __global__ void __launch_bounds__(BLOCK_THREADS, 1)
-k_substeps(EngineDev e, const int* __restrict__ block_model, const int* __restrict__ block_start, const int* __restrict__ block_count,
-           const int* __restrict__ perm, int nstep, float c0, float c1, float* __restrict__ dump) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  BlockShared* bs = (BlockShared*)smem;
-  WarpShared* wsa = (WarpShared*)(smem + sizeof(BlockShared));
-  const int mi = block_model[blockIdx.x];
-  stage_model(bs, e.models + (size_t)mi * e.model_stride, (unsigned)sizeof(bs->model), e.taskconsts + mi);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp >= block_count[blockIdx.x]) return;
-  const int env = perm[block_start[blockIdx.x] + warp];
-  WarpShared* ws = wsa + warp;
-  ws->w.epa = e.epa + scratch_slot(e, warp);
-  ws->w.sp = e.spill + scratch_slot(e, warp);
-  join_cta(bs, wsa, &ws->w, warp, block_count[blockIdx.x]);
-  const MwModel* m = (const MwModel*)bs->model;
+k_substeps(EngineDev e, BlockTable bt, int nstep, float c0, float c1, float* __restrict__ dump) {
+  CtaWarp cw;
+  if (!cta_enter(e, bt, blockIdx.x, cw)) return;
+  WarpShared* ws = cw.ws; const MwModel* m = cw.m;
+  const int mi = cw.mi, lane = cw.lane, env = cw.env;
   load_env(ws, e.state + env, lane);
   if (lane == 0) { ws->w.ctrl[0] = c0; ws->w.ctrl[1] = c1; }
   SYNCW();
@@ -435,30 +458,18 @@ k_substeps(EngineDev e, const int* __restrict__ block_model, const int* __restri
 // evaluate_state (sawyer_xyz_env.py:644-656 + the task's compute_reward): reward / info of the CURRENT state for a given
 // (obs, action); one forward pass to rebuild poses and contact forces, nothing is written back to the state
 __global__ void __launch_bounds__(BLOCK_THREADS, 1)
-k_evaluate(EngineDev e, const int* __restrict__ block_model, const int* __restrict__ block_start, const int* __restrict__ block_count,
-           const int* __restrict__ perm, const float* __restrict__ actions, const float* __restrict__ obs_in, int obs_stride, float* __restrict__ out) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  BlockShared* bs = (BlockShared*)smem;
-  WarpShared* wsa = (WarpShared*)(smem + sizeof(BlockShared));
-  const int mi = block_model[blockIdx.x];
-  stage_model(bs, e.models + (size_t)mi * e.model_stride, (unsigned)sizeof(bs->model), e.taskconsts + mi);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp >= block_count[blockIdx.x]) return;
-  const int env = perm[block_start[blockIdx.x] + warp];
-  WarpShared* ws = wsa + warp;
-  ws->w.epa = e.epa + scratch_slot(e, warp);
-  ws->w.sp = e.spill + scratch_slot(e, warp);
-  WarpScratch* w = &ws->w;
-  join_cta(bs, wsa, w, warp, block_count[blockIdx.x]);
-  const MwModel* m = (const MwModel*)bs->model;
-  load_env(ws, e.state + env, lane);
-  if (lane < 16) w->prof[lane] = 0;
-  if (lane == 0) { w->fault = 0; w->prof_on = 0; w->ctrl[0] = actions[4 * env + 3]; w->ctrl[1] = -actions[4 * env + 3]; }
+k_evaluate(EngineDev e, BlockTable bt, const float* __restrict__ actions, const float* __restrict__ obs_in, int obs_stride, float* __restrict__ out) {
+  CtaWarp cw;
+  if (!cta_enter(e, bt, blockIdx.x, cw)) return;
+  WarpScratch* w = cw.w;
+  const int lane = cw.lane, env = cw.env;
+  enter_env(e, cw, 0);
+  if (lane == 0) { w->ctrl[0] = actions[4 * env + 3]; w->ctrl[1] = -actions[4 * env + 3]; }
   SYNCW();
-  mw_forward(m, e.meshverts[mi], w, lane);
+  mw_forward(cw.m, e.meshverts[cw.mi], w, lane);
   if (lane == 0) {
     real raw_act[4]; for (int i = 0; i < 4; i++) raw_act[i] = actions[4 * env + i];
-    TaskCtx c; c.m = m; c.tc = &bs->tc; c.w = w; c.s = &ws->es; c.action = raw_act; c.meshvert = e.meshverts[mi];
+    TaskCtx c = task_ctx(e, cw, raw_act);
     task_live_update(c);
     real obsr[39]; for (int i = 0; i < 39; i++) obsr[i] = obs_in[(size_t)env * obs_stride + i];
     real rew, inf[INFO_N];
@@ -507,41 +518,21 @@ __global__ void k_expert(int n, const int* __restrict__ task_ids, const float* _
 // SawyerXYZEnv._get_obs (sawyer_xyz_env.py:513-527) of the current state for the envs with mask[env] set: the kinematics
 // pass, then the unclipped observation; commits prev_obs (the frame stack) like the reference.  No task's observation
 // reads contacts or forces (task_obs_objects: frame poses and qpos only), so the kinematics pass is all of mj_forward
-// that it needs.  Barriers: a CTA whose envs are all unmasked leaves before its first barrier (every thread of the CTA
-// reads the same mask bytes, so the exit is uniform); in a CTA that stays, the unmasked warps run the same kinematics
-// pass as the masked ones and so meet every barrier (the one at the start of mw_forward_kinematics_only), and only
-// skip the writes; warps past block_count exit before any barrier and are not counted by it (as in k_step).
+// that it needs.  Barriers: see cta_has_masked; the one that the unmasked warps meet is at the start of
+// mw_forward_kinematics_only.
 __global__ void __launch_bounds__(BLOCK_THREADS, 1)
-k_observe(EngineDev e, const int* __restrict__ block_model, const int* __restrict__ block_start, const int* __restrict__ block_count,
-          const int* __restrict__ perm, const unsigned char* __restrict__ mask, float* __restrict__ obs_out, int obs_stride) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  BlockShared* bs = (BlockShared*)smem;
-  WarpShared* wsa = (WarpShared*)(smem + sizeof(BlockShared));
-  {
-    bool any = false;
-    for (int k = 0; k < block_count[blockIdx.x]; k++) any = any || mask[perm[block_start[blockIdx.x] + k]];
-    if (!any) return;
-  }
-  const int mi = block_model[blockIdx.x];
-  stage_model(bs, e.models + (size_t)mi * e.model_stride, (unsigned)sizeof(bs->model), e.taskconsts + mi);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp >= block_count[blockIdx.x]) return;
-  const int env = perm[block_start[blockIdx.x] + warp];
-  WarpShared* ws = wsa + warp;
-  ws->w.epa = e.epa + scratch_slot(e, warp);
-  ws->w.sp = e.spill + scratch_slot(e, warp);
-  WarpScratch* w = &ws->w;
-  join_cta(bs, wsa, w, warp, block_count[blockIdx.x]);
-  const MwModel* m = (const MwModel*)bs->model;
-  load_env(ws, e.state + env, lane);
-  if (lane < 16) w->prof[lane] = 0;
-  if (lane == 0) { w->fault = 0; w->prof_on = 0; }
-  SYNCW();
-  mw_forward_kinematics_only(m, w, lane);
+k_observe(EngineDev e, BlockTable bt, const unsigned char* __restrict__ mask, float* __restrict__ obs_out, int obs_stride) {
+  if (!cta_has_masked(bt, blockIdx.x, mask)) return;
+  CtaWarp cw;
+  if (!cta_enter(e, bt, blockIdx.x, cw)) return;
+  WarpShared* ws = cw.ws;
+  const int lane = cw.lane, env = cw.env;
+  enter_env(e, cw, 0);
+  mw_forward_kinematics_only(cw.m, cw.w, lane);
   if (!mask[env]) return;                              // after the CTA's last barrier
   if (lane == 0) {
     real act[4] = {0, 0, 0, 0};
-    TaskCtx c; c.m = m; c.tc = &bs->tc; c.w = w; c.s = &ws->es; c.action = act; c.meshvert = e.meshverts[mi];
+    TaskCtx c = task_ctx(e, cw, act);
     task_live_update(c);                               // _target_pos of the tasks that alias a site (as k_step before make_obs)
     make_obs(c, ws->obs, /*clip=*/false);
     bool fin = true; for (int i = 0; i < 39; i++) fin = fin && isfinite(ws->obs[i]);
@@ -567,43 +558,25 @@ static_assert(sizeof(MwQueryFrame) == 64, "MwQueryFrame layout mismatch with low
 // Read-only state query of the envs with mask[env] set (mw_query): the current observation frame (columns 0..17 of the next
 // _get_obs, unclipped), world poses of named frames and touching_object of one collider.  Nothing is written back: not the
 // record (the frame stack, the live target), the warm start, the separating-axis hints (join_cta without hints) or any fault
-// bit but MW_FAULT_NONFINITE.  Barriers as in k_observe: a CTA without a masked env leaves before its first barrier, the
-// unmasked warps of a CTA that stays run the same pass and skip the writes, warps past block_count exit before any barrier.
-// `touch_geom` non-null: the full forward pass (contacts, constraint forces from the record's gripper command), else the
-// kinematics pass only.
+// bit but MW_FAULT_NONFINITE.  Barriers: see cta_has_masked.  `touch_geom` non-null: the full forward pass (contacts,
+// constraint forces from the record's gripper command), else the kinematics pass only.
 __global__ void __launch_bounds__(BLOCK_THREADS, 1)
-k_query(EngineDev e, const int* __restrict__ block_model, const int* __restrict__ block_start, const int* __restrict__ block_count,
-        const int* __restrict__ perm, const unsigned char* __restrict__ mask, float* __restrict__ frame_out,
+k_query(EngineDev e, BlockTable bt, const unsigned char* __restrict__ mask, float* __restrict__ frame_out,
         const MwQueryFrame* __restrict__ table, int nq_frames, double* __restrict__ pose_out,
         const int* __restrict__ touch_geom, unsigned char* __restrict__ touching_out) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  BlockShared* bs = (BlockShared*)smem;
-  WarpShared* wsa = (WarpShared*)(smem + sizeof(BlockShared));
-  {
-    bool any = false;
-    for (int k = 0; k < block_count[blockIdx.x]; k++) any = any || mask[perm[block_start[blockIdx.x] + k]];
-    if (!any) return;
-  }
-  const int mi = block_model[blockIdx.x];
-  stage_model(bs, e.models + (size_t)mi * e.model_stride, (unsigned)sizeof(bs->model), e.taskconsts + mi);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp >= block_count[blockIdx.x]) return;
-  const int env = perm[block_start[blockIdx.x] + warp];
-  WarpShared* ws = wsa + warp;
-  ws->w.epa = e.epa + scratch_slot(e, warp);
-  ws->w.sp = e.spill + scratch_slot(e, warp);
-  WarpScratch* w = &ws->w;
-  join_cta(bs, wsa, w, warp, block_count[blockIdx.x]);
-  const MwModel* m = (const MwModel*)bs->model;
-  load_env(ws, e.state + env, lane);
-  if (lane < 16) w->prof[lane] = 0;
-  if (lane == 0) { w->fault = 0; w->prof_on = 0; w->ctrl[0] = ws->es.gripper_ctrl; w->ctrl[1] = -ws->es.gripper_ctrl; }
+  if (!cta_has_masked(bt, blockIdx.x, mask)) return;
+  CtaWarp cw;
+  if (!cta_enter(e, bt, blockIdx.x, cw)) return;
+  BlockShared* bs = cw.bs; WarpShared* ws = cw.ws; WarpScratch* w = cw.w;
+  const int mi = cw.mi, lane = cw.lane, env = cw.env;
+  enter_env(e, cw, 0);
+  if (lane == 0) { w->ctrl[0] = ws->es.gripper_ctrl; w->ctrl[1] = -ws->es.gripper_ctrl; }
   SYNCW();
-  if (touching_out) mw_forward(m, e.meshverts[mi], w, lane);
-  else mw_forward_kinematics_only(m, w, lane);
+  if (touching_out) mw_forward(cw.m, e.meshverts[mi], w, lane);
+  else mw_forward_kinematics_only(cw.m, w, lane);
   if (!mask[env]) return;                              // after the CTA's last barrier
   real act[4] = {0, 0, 0, 0};
-  TaskCtx c; c.m = m; c.tc = &bs->tc; c.w = w; c.s = &ws->es; c.action = act; c.meshvert = e.meshverts[mi];
+  TaskCtx c = task_ctx(e, cw, act);
   if (lane == 0) {
     task_live_update(c);                               // basketball's aliased goal, as before make_obs in k_step
     if (frame_out) {
@@ -766,6 +739,7 @@ struct mw_engine {
     e.sep_hint = d_sep_hint;
     e.n_envs = n_envs; e.max_steps = max_steps; e.terminate_on_success = terminate_on_success; e.seed = seed; e.autoreset_mode = autoreset_mode; return e;
   }
+  BlockTable blocks() const { return {d_block_model, d_block_start, d_block_count, d_perm}; }
 };
 
 // group work items by model into CTAs of WARPS_PER_BLOCK warps
@@ -984,7 +958,7 @@ int mw_build_snapshots(mw_engine* E, int n, const int* model_idx, const double* 
   CK(cudaMalloc((void**)&d_po, n)); CK(cudaMemcpy(d_po, partial, n, cudaMemcpyHostToDevice));
   double* d_rv1 = nullptr;
   if (rand_vec_pass1) { CK(cudaMalloc((void**)&d_rv1, sizeof(double) * 6 * n)); CK(cudaMemcpy(d_rv1, rand_vec_pass1, sizeof(double) * 6 * n, cudaMemcpyHostToDevice)); }
-  k_snapshot<<<(int)bm.size(), BLOCK_THREADS, smem_bytes()>>>(E->dev(), d_bm, d_bs, d_bc, d_perm, d_rv, d_rv1, d_po, E->n_snaps);
+  k_snapshot<<<(int)bm.size(), BLOCK_THREADS, smem_bytes()>>>(E->dev(), BlockTable{d_bm, d_bs, d_bc, d_perm}, d_rv, d_rv1, d_po, E->n_snaps);
   CK(cudaGetLastError());
   CK(cudaDeviceSynchronize());
   cudaFree(d_bm); cudaFree(d_bs); cudaFree(d_bc); cudaFree(d_perm); cudaFree(d_rv); cudaFree(d_rv1); cudaFree(d_po);
@@ -1059,7 +1033,7 @@ int mw_step(mw_engine* E, const float* actions, float* obs, int obs_stride, floa
         E->n_blocks, E->n_split, E->d_split_head, E->d_split_alt, E->d_split_state, E->n_split ? E->d_block_live : nullptr, E->split_frac, E->n_sm);
   }
   auto* kern = E->autoreset_mode == MW_AUTORESET_SAME_STEP ? k_step<false> : k_step<true>;
-  kern<<<E->n_split ? E->n_blocks_total : E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_order, E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm,
+  kern<<<E->n_split ? E->n_blocks_total : E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_order, E->blocks(),
       actions, obs, obs_stride, reward, terminated, truncated, info, info_stride, final_obs, final_info, next_snapshot, E->n_split ? E->d_block_live : nullptr);
   CK(cudaGetLastError());
   E->launches += 3; E->env_steps += (unsigned long long)E->n_envs;
@@ -1069,7 +1043,7 @@ int mw_step(mw_engine* E, const float* actions, float* obs, int obs_stride, floa
 int mw_evaluate(mw_engine* E, const float* actions, const float* obs, int obs_stride, float* out, void* stream) {
   if (!E || !E->d_state || !actions || !obs || !out || obs_stride < 39) return fail(MW_ERR_ARG, "mw_evaluate: bad arguments");
   CK(cudaSetDevice(E->device));
-  k_evaluate<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm, actions, obs, obs_stride, out);
+  k_evaluate<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), actions, obs, obs_stride, out);
   CK(cudaGetLastError());
   E->launches++;
   return MW_OK;
@@ -1099,7 +1073,7 @@ int mw_observe(mw_engine* E, const unsigned char* mask, float* obs, int obs_stri
   if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_observe: mw_set_envs not called");
   if (!mask || !obs || obs_stride < 39) return fail(MW_ERR_ARG, "mw_observe: bad arguments");
   CK(cudaSetDevice(E->device));
-  k_observe<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm, mask, obs, obs_stride);
+  k_observe<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), mask, obs, obs_stride);
   CK(cudaGetLastError());
   E->launches++;
   return MW_OK;
@@ -1112,8 +1086,7 @@ int mw_query(mw_engine* E, const unsigned char* mask, float* frame, const void* 
     return fail(MW_ERR_ARG, "mw_query: bad arguments");
   if (!frame && !pose && !touching) return MW_OK;
   CK(cudaSetDevice(E->device));
-  k_query<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm,
-      mask, frame, (const MwQueryFrame*)frames, pose ? n_frames : 0, pose, touch_geom, touching);
+  k_query<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), mask, frame, (const MwQueryFrame*)frames, pose ? n_frames : 0, pose, touch_geom, touching);
   CK(cudaGetLastError());
   E->launches++;
   return MW_OK;
@@ -1165,7 +1138,7 @@ int mw_set_state(mw_engine* E, const void* in) {
 int mw_debug_substeps(mw_engine* E, int nstep, const float* ctrl2, void* stream) {
   if (!E || !E->d_state || nstep < 0 || !ctrl2) return fail(MW_ERR_ARG, "mw_debug_substeps");
   CK(cudaSetDevice(E->device));
-  k_substeps<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm, nstep, ctrl2[0], ctrl2[1], nullptr);
+  k_substeps<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), nstep, ctrl2[0], ctrl2[1], nullptr);
   CK(cudaGetLastError());
   E->launches++;
   return MW_OK;
@@ -1173,7 +1146,7 @@ int mw_debug_substeps(mw_engine* E, int nstep, const float* ctrl2, void* stream)
 int mw_debug_forward(mw_engine* E, const float* ctrl2, float* dump_dev, void* stream) {
   if (!E || !E->d_state || !ctrl2 || !dump_dev) return fail(MW_ERR_ARG, "mw_debug_forward");
   CK(cudaSetDevice(E->device));
-  k_substeps<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_model, E->d_block_start, E->d_block_count, E->d_perm, 0, ctrl2[0], ctrl2[1], dump_dev);
+  k_substeps<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), 0, ctrl2[0], ctrl2[1], dump_dev);
   CK(cudaGetLastError());
   return MW_OK;
 }
