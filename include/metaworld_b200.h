@@ -202,7 +202,8 @@ int mw_get_env_profile(mw_engine*, unsigned* out /*host [n_envs*20]*/);
  * waiting for the CTA's other warps at phase boundaries (not part of [0]..[7]); [13] GJK/EPA pairs tested against their
  * separating-axis hint, [14] of those, pairs the hint proved apart (no GJK/EPA run; [2] and [9] include them) */
 int mw_get_profile(mw_engine*, unsigned long long* out15);
-/* warp cycles each environment spent in its most recent step (host array of n_envs) */
+/* solver work of each environment's most recent step (host array of n_envs): the estimate, from Newton iterations weighted
+ * by the constraint rows they touch, that orders a model's environments for the next launch (costliest first)       */
 int mw_get_env_cost(mw_engine*, unsigned* out);
 
 #ifdef __cplusplus

@@ -12,6 +12,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 #include <string>
 #include <utility>
 #include <vector>
@@ -713,33 +714,68 @@ __global__ void k_order_blocks(int n_blocks, const int* __restrict__ block_start
 }
 
 // ---------------------------------------------------------------- host side
+// One device array and its length.  The destructor frees it, so a buffer is released on every return path of the entry
+// point that holds it.  alloc and upload replace the contents only when every CUDA call succeeded.  Callers select the
+// engine's device first.
+template <class T> struct DevBuf {
+  T* p = nullptr; size_t n = 0;
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(n, o.n); return *this; }   // o frees the old array
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { cudaFree(p); }
+  cudaError_t alloc(size_t count, bool zero = false) {
+    DevBuf b;
+    cudaError_t e = cudaMalloc((void**)&b.p, sizeof(T) * count);
+    if (e == cudaSuccess) { b.n = count; if (zero) e = cudaMemset(b.p, 0, sizeof(T) * count); }
+    if (e == cudaSuccess) *this = std::move(b);
+    return e;
+  }
+  // host -> device; at least one element is allocated, so that an empty table is a valid pointer
+  cudaError_t upload(const T* src, size_t count) {
+    DevBuf b;
+    cudaError_t e = b.alloc(count ? count : 1);
+    if (e == cudaSuccess && count) e = cudaMemcpy(b.p, src, sizeof(T) * count, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) *this = std::move(b);
+    return e;
+  }
+  cudaError_t upload(const std::vector<T>& v) { return upload(v.data(), v.size()); }
+};
+
+// The CTA table of the environment set, then the buffers of the launch-order kernels (k_order_envs / k_order_blocks)
+struct EnvBlocks {
+  int n_blocks = 0, n_blocks_total = 0, n_split = 0, n_sorted_models = 0;
+  DevBuf<int> model, start, count, perm;           // head split: the alternative CTAs follow the n_blocks regular ones
+  DevBuf<int> model_first, model_count, order;
+  DevBuf<int> split_head, split_alt, split_state, live;
+};
+
 struct mw_engine {
   int device = 0, n_models = 0, n_envs = 0, model_stride = 0;
-  unsigned char* d_models = nullptr; MwTaskConst* d_tc = nullptr; float** d_meshptrs = nullptr;
-  std::vector<float*> meshbufs;
-  MwEnvState* d_state = nullptr; MwSnapshot* d_snaps = nullptr; int snap_cap = 0, n_snaps = 0;
-  int *d_goal_first = nullptr, *d_goal_count = nullptr, *d_diag = nullptr;
-  EpaWs* d_epa = nullptr; WarpSpill* d_spill = nullptr; size_t epa_cap = 0; int slot_by_sm = 0, nsmid = 0;
-  unsigned long long* d_prof = nullptr; unsigned long long* d_model_cycles = nullptr; unsigned* d_env_prof = nullptr; int profiling = 0;
-  float4* d_sep_hint = nullptr;
-  unsigned* d_env_cost = nullptr; unsigned* d_env_cycles = nullptr; int order_by_cycles = 1, head_warps = 0; int *d_block_order = nullptr, *d_model_first = nullptr, *d_model_count = nullptr; int n_sorted_models = 0;
+  DevBuf<unsigned char> d_models; DevBuf<MwTaskConst> d_tc; DevBuf<float*> d_meshptrs;
+  std::vector<DevBuf<float>> meshbufs;
+  DevBuf<MwEnvState> d_state; DevBuf<MwSnapshot> d_snaps; int n_snaps = 0;
+  DevBuf<int> d_goal_first, d_goal_count, d_diag;
+  DevBuf<EpaWs> d_epa; DevBuf<WarpSpill> d_spill; int slot_by_sm = 0, nsmid = 0;
+  DevBuf<unsigned long long> d_prof, d_model_cycles; DevBuf<unsigned> d_env_prof; int profiling = 0;
+  DevBuf<float4> d_sep_hint;
+  DevBuf<unsigned> d_env_cost, d_env_cycles; int order_by_cycles = 1, head_warps = 0;
   std::vector<int> h_faults;                                   // fault bits already drained from d_diag by mw_get_counters
   std::vector<int> env_model; std::vector<int> model_order;   // block table inputs (mw_rebalance re-sorts the models by measured cost)
-  int* d_env_model = nullptr;                                  // env_model on the device (k_set_physics / k_get_physics read each env's nq / nv)
-  // env block table
-  int n_blocks = 0; int *d_block_model = nullptr, *d_block_start = nullptr, *d_block_count = nullptr, *d_perm = nullptr;
-  // head split (k_order_blocks): the alternative CTAs follow the n_blocks regular ones in the block table
-  int n_blocks_total = 0, n_split = 0, split_warps = 4, n_sm = 0; float split_frac = 0.f;
-  int *d_split_head = nullptr, *d_split_alt = nullptr, *d_split_state = nullptr, *d_block_live = nullptr;
+  DevBuf<int> d_env_model;                                     // env_model on the device (k_set_physics / k_get_physics read each env's nq / nv)
+  EnvBlocks blk;
+  // head split (k_order_blocks)
+  int split_warps = 4, n_sm = 0; float split_frac = 0.f;
   int max_steps = 500, terminate_on_success = 0; unsigned long long seed = 0; int autoreset_mode = MW_AUTORESET_SAME_STEP;
   unsigned long long launches = 0, env_steps = 0;
   EngineDev dev() const {
-    EngineDev e; e.models = d_models; e.model_stride = model_stride; e.taskconsts = d_tc; e.meshverts = d_meshptrs;
-    e.state = d_state; e.snaps = d_snaps; e.goal_first = d_goal_first; e.goal_count = d_goal_count; e.diag = d_diag; e.epa = d_epa; e.spill = d_spill; e.slot_by_sm = slot_by_sm; e.prof = profiling ? d_prof : nullptr; e.model_cycles = d_model_cycles; e.env_cost = d_env_cost; e.env_cycles = order_by_cycles ? d_env_cycles : nullptr; e.env_prof = profiling ? d_env_prof : nullptr;
-    e.sep_hint = d_sep_hint;
+    EngineDev e; e.models = d_models.p; e.model_stride = model_stride; e.taskconsts = d_tc.p; e.meshverts = d_meshptrs.p;
+    e.state = d_state.p; e.snaps = d_snaps.p; e.goal_first = d_goal_first.p; e.goal_count = d_goal_count.p; e.diag = d_diag.p; e.epa = d_epa.p; e.spill = d_spill.p; e.slot_by_sm = slot_by_sm; e.prof = profiling ? d_prof.p : nullptr; e.model_cycles = d_model_cycles.p; e.env_cost = d_env_cost.p; e.env_cycles = order_by_cycles ? d_env_cycles.p : nullptr; e.env_prof = profiling ? d_env_prof.p : nullptr;
+    e.sep_hint = d_sep_hint.p;
     e.n_envs = n_envs; e.max_steps = max_steps; e.terminate_on_success = terminate_on_success; e.seed = seed; e.autoreset_mode = autoreset_mode; return e;
   }
-  BlockTable blocks() const { return {d_block_model, d_block_start, d_block_count, d_perm}; }
+  BlockTable blocks() const { return {blk.model.p, blk.start.p, blk.count.p, blk.perm.p}; }
 };
 
 // group work items by model into CTAs of WARPS_PER_BLOCK warps
@@ -772,36 +808,29 @@ static int ensure_epa(mw_engine* E, size_t n_blocks) {
   if (E->nsmid == 0) {
     // one CTA per SM whenever two CTAs' shared memory cannot fit (true for every build so far: 190-227 KB per CTA)
     int dev = 0; cudaDeviceProp pr; CK(cudaGetDevice(&dev)); CK(cudaGetDeviceProperties(&pr, dev));
-    unsigned* d_n = nullptr; unsigned h_n = 0;
-    CK(cudaMalloc((void**)&d_n, sizeof(unsigned)));
-    k_nsmid<<<1, 1>>>(d_n);
-    CK(cudaMemcpy(&h_n, d_n, sizeof(unsigned), cudaMemcpyDeviceToHost)); cudaFree(d_n);
+    DevBuf<unsigned> d_n; unsigned h_n = 0;
+    CK(d_n.alloc(1));
+    k_nsmid<<<1, 1>>>(d_n.p);
+    CK(cudaMemcpy(&h_n, d_n.p, sizeof(unsigned), cudaMemcpyDeviceToHost));
     E->nsmid = (int)h_n;
     E->slot_by_sm = (2 * smem_bytes() > (size_t)pr.sharedMemPerMultiprocessor && h_n > 0 && h_n <= 4096) ? 1 : 0;
   }
   size_t need = (E->slot_by_sm ? (size_t)E->nsmid : n_blocks) * WARPS_PER_BLOCK;
-  if (need <= E->epa_cap) return 0;
-  if (E->d_epa) cudaFree(E->d_epa);
-  if (E->d_spill) cudaFree(E->d_spill);
-  E->d_epa = nullptr; E->d_spill = nullptr; E->epa_cap = 0;
-  CK(cudaMalloc((void**)&E->d_epa, sizeof(EpaWs) * need));
-  CK(cudaMalloc((void**)&E->d_spill, sizeof(WarpSpill) * need));
-  E->epa_cap = need;
-  return 0;
-}
-template <class T> static int upload(T** dst, const std::vector<T>& v) {
-  if (*dst) cudaFree(*dst);
-  *dst = nullptr;
-  CK(cudaMalloc((void**)dst, sizeof(T) * (v.size() ? v.size() : 1)));
-  if (!v.empty()) CK(cudaMemcpy(*dst, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice));
+  if (need <= E->d_epa.n) return 0;
+  DevBuf<EpaWs> epa; DevBuf<WarpSpill> spill;
+  CK(epa.alloc(need));
+  CK(spill.alloc(need));
+  E->d_epa = std::move(epa); E->d_spill = std::move(spill);
   return 0;
 }
 
-// (re)builds and uploads the CTA table of the environment set + the buffers of the launch-order kernels
-static int upload_env_blocks(mw_engine* E) {
+// builds and uploads the CTA table of `env_model` (models launched in `model_order`) + the buffers of the launch-order
+// kernels into `out`; E keeps its own table
+static int upload_env_blocks(mw_engine* E, const std::vector<int>& env_model, const std::vector<int>& model_order, EnvBlocks& out) {
   std::vector<int> bm, bs, bc, perm;
-  make_blocks(E->n_models, E->env_model, bm, bs, bc, perm, &E->model_order, E->head_warps);
-  E->n_blocks = (int)bm.size();
+  make_blocks(E->n_models, env_model, bm, bs, bc, perm, &model_order, E->head_warps);
+  EnvBlocks t;
+  t.n_blocks = (int)bm.size();
   std::vector<int> mfirst, mcount;
   for (size_t b = 0; b < bm.size(); b++) {
     if (b == 0 || bm[b] != bm[b - 1]) { mfirst.push_back(bs[b]); mcount.push_back(0); }
@@ -820,15 +849,44 @@ static int upload_env_blocks(mw_engine* E) {
       }
     }
   }
-  E->n_split = (int)shead.size(); E->n_blocks_total = (int)bm.size();
+  t.n_split = (int)shead.size(); t.n_blocks_total = (int)bm.size();
   if (ensure_epa(E, bm.size())) return MW_ERR_CUDA;
-  if (upload(&E->d_block_model, bm) || upload(&E->d_block_start, bs) || upload(&E->d_block_count, bc) || upload(&E->d_perm, perm)) return MW_ERR_CUDA;
+  CK(t.model.upload(bm)); CK(t.start.upload(bs)); CK(t.count.upload(bc)); CK(t.perm.upload(perm));
   std::vector<int> order(bm.size()), live(bm.size()), zero(shead.size() ? shead.size() : 1, 0);
-  for (size_t b = 0; b < bm.size(); b++) { order[b] = (int)b; live[b] = b < (size_t)E->n_blocks; }
-  E->n_sorted_models = (int)mfirst.size();
-  if (upload(&E->d_model_first, mfirst) || upload(&E->d_model_count, mcount) || upload(&E->d_block_order, order)) return MW_ERR_CUDA;
-  if (upload(&E->d_split_head, shead) || upload(&E->d_split_alt, salt) || upload(&E->d_split_state, zero) || upload(&E->d_block_live, live)) return MW_ERR_CUDA;
+  for (size_t b = 0; b < bm.size(); b++) { order[b] = (int)b; live[b] = b < (size_t)t.n_blocks; }
+  t.n_sorted_models = (int)mfirst.size();
+  CK(t.model_first.upload(mfirst)); CK(t.model_count.upload(mcount)); CK(t.order.upload(order));
+  CK(t.split_head.upload(shead)); CK(t.split_alt.upload(salt)); CK(t.split_state.upload(zero)); CK(t.live.upload(live));
+  out = std::move(t);
   return 0;
+}
+
+// grows the snapshot table so that n more records fit (to twice the records then held)
+static int reserve_snapshots(mw_engine* E, int n) {
+  if ((size_t)(E->n_snaps + n) <= E->d_snaps.n) return 0;
+  DevBuf<MwSnapshot> t;
+  CK(t.alloc((size_t)(E->n_snaps + n) * 2));
+  if (E->n_snaps) CK(cudaMemcpy(t.p, E->d_snaps.p, sizeof(MwSnapshot) * E->n_snaps, cudaMemcpyDeviceToDevice));
+  E->d_snaps = std::move(t);
+  return 0;
+}
+
+// d_diag on the host: [n_envs][3] = contacts dropped, solver iterations, MW_FAULT_* bits
+static int read_diag(const mw_engine* E, std::vector<int>& diag) {
+  diag.assign(3 * (size_t)E->n_envs, 0);
+  if (!diag.empty()) CK(cudaMemcpy(diag.data(), E->d_diag.p, sizeof(int) * diag.size(), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// one warp per row (k_reset, k_reset_masked, k_set_physics, k_get_physics)
+#define ROW_THREADS 256
+static int row_blocks(int rows) { return (rows * 32 + ROW_THREADS - 1) / ROW_THREADS; }
+
+// the end of an entry point that queued `n` kernels: reports a failed launch, else counts them (mw_get_counters [0])
+static int launched(mw_engine* E, int n) {
+  CK(cudaGetLastError());
+  E->launches += n;
+  return MW_OK;
 }
 
 extern "C" {
@@ -851,33 +909,26 @@ int mw_create(mw_engine** out, int device, int n_models, const void* models, con
   CK(cudaGetDeviceCount(&ndev));
   if (device < 0 || device >= ndev) return fail(MW_ERR_CUDA, "mw_create: no such CUDA device (this engine has no CPU path)");
   CK(cudaSetDevice(device));
-  mw_engine* E = new mw_engine();
+  std::unique_ptr<mw_engine> E(new mw_engine());
   E->device = device; E->n_models = n_models;
   E->model_stride = (int)((sizeof(MwModel) + 15) / 16 * 16);
   std::vector<unsigned char> blob((size_t)E->model_stride * n_models, 0);
   for (int i = 0; i < n_models; i++) memcpy(blob.data() + (size_t)i * E->model_stride, (const unsigned char*)models + (size_t)i * sizeof(MwModel), sizeof(MwModel));
-  CK(cudaMalloc((void**)&E->d_models, blob.size()));
-  CK(cudaMemcpy(E->d_models, blob.data(), blob.size(), cudaMemcpyHostToDevice));
-  CK(cudaMalloc((void**)&E->d_tc, sizeof(MwTaskConst) * n_models));
-  CK(cudaMemcpy(E->d_tc, taskconsts, sizeof(MwTaskConst) * n_models, cudaMemcpyHostToDevice));
+  CK(E->d_models.upload(blob));
+  CK(E->d_tc.upload((const MwTaskConst*)taskconsts, n_models));
   std::vector<float*> ptrs(n_models, nullptr);
+  E->meshbufs.resize(n_models);
   for (int i = 0; i < n_models; i++) {
     int nvt = nmeshvert ? nmeshvert[i] : 0;
-    float* p = nullptr;
-    CK(cudaMalloc((void**)&p, sizeof(float) * 4 * (nvt > 0 ? nvt : 1)));
-    if (nvt > 0) {   // repack xyz -> xyz_ so that a support query reads one 16-byte word per vertex
-      std::vector<float> packed(4 * (size_t)nvt, 0.f);
-      for (int v = 0; v < nvt; v++) for (int c = 0; c < 3; c++) packed[4 * v + c] = meshverts[i][3 * v + c];
-      CK(cudaMemcpy(p, packed.data(), sizeof(float) * 4 * nvt, cudaMemcpyHostToDevice));
-    }
-    ptrs[i] = p; E->meshbufs.push_back(p);
+    // repack xyz -> xyz_ so that a support query reads one 16-byte word per vertex
+    std::vector<float> packed(4 * (size_t)(nvt > 0 ? nvt : 1), 0.f);
+    for (int v = 0; v < nvt; v++) for (int c = 0; c < 3; c++) packed[4 * v + c] = meshverts[i][3 * v + c];
+    CK(E->meshbufs[i].upload(packed));
+    ptrs[i] = E->meshbufs[i].p;
   }
-  CK(cudaMalloc((void**)&E->d_meshptrs, sizeof(float*) * n_models));
-  CK(cudaMemcpy(E->d_meshptrs, ptrs.data(), sizeof(float*) * n_models, cudaMemcpyHostToDevice));
-  CK(cudaMalloc((void**)&E->d_model_cycles, sizeof(unsigned long long) * 2 * n_models));
-  CK(cudaMemset(E->d_model_cycles, 0, sizeof(unsigned long long) * 2 * n_models));
-  CK(cudaMalloc((void**)&E->d_prof, sizeof(unsigned long long) * 16));
-  CK(cudaMemset(E->d_prof, 0, sizeof(unsigned long long) * 16));
+  CK(E->d_meshptrs.upload(ptrs));
+  CK(E->d_model_cycles.alloc(2 * (size_t)n_models, true));
+  CK(E->d_prof.alloc(16, true));
   CK(cudaFuncSetAttribute(k_order_envs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(unsigned long long) * MW_SORT_MAX)));
   CK(cudaFuncSetAttribute(k_order_blocks, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(unsigned long long) * MW_SORT_MAX)));
   CK(cudaFuncSetAttribute(k_step<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
@@ -892,76 +943,59 @@ int mw_create(mw_engine** out, int device, int n_models, const void* models, con
   { const char* k = getenv("MW_B200_SPLIT_FRAC"); if (k) E->split_frac = (float)atof(k); }
   { const char* k = getenv("MW_B200_SPLIT_WARPS"); if (k) E->split_warps = atoi(k); }
   { cudaDeviceProp pr; CK(cudaGetDeviceProperties(&pr, device)); E->n_sm = pr.multiProcessorCount; }
-  *out = E;
+  *out = E.release();
   return MW_OK;
 }
 
 void mw_destroy(mw_engine* E) {
   if (!E) return;
   cudaSetDevice(E->device);
-  cudaFree(E->d_models); cudaFree(E->d_tc); cudaFree(E->d_meshptrs);
-  for (float* p : E->meshbufs) cudaFree(p);
-  cudaFree(E->d_state); cudaFree(E->d_snaps); cudaFree(E->d_goal_first); cudaFree(E->d_goal_count); cudaFree(E->d_diag); cudaFree(E->d_epa); cudaFree(E->d_spill); cudaFree(E->d_prof); cudaFree(E->d_model_cycles); cudaFree(E->d_env_prof); cudaFree(E->d_env_cost); cudaFree(E->d_env_cycles); cudaFree(E->d_sep_hint); cudaFree(E->d_env_model); cudaFree(E->d_block_order); cudaFree(E->d_model_first); cudaFree(E->d_model_count);
-  cudaFree(E->d_block_model); cudaFree(E->d_block_start); cudaFree(E->d_block_count); cudaFree(E->d_perm);
-  cudaFree(E->d_split_head); cudaFree(E->d_split_alt); cudaFree(E->d_split_state); cudaFree(E->d_block_live);
   delete E;
 }
 
 int mw_set_envs(mw_engine* E, int n_envs, const int* env_model) {
   if (!E || n_envs <= 0 || !env_model) return fail(MW_ERR_ARG, "mw_set_envs: bad arguments");
   CK(cudaSetDevice(E->device));
-  std::vector<int> im(env_model, env_model + n_envs), bm, bs, bc, perm;
+  std::vector<int> im(env_model, env_model + n_envs);
   for (int v : im) if (v < 0 || v >= E->n_models) return fail(MW_ERR_ARG, "mw_set_envs: model index out of range");
+  // everything is built aside and replaces the engine's tables only once every allocation has succeeded
+  EnvBlocks blk;
+  if (upload_env_blocks(E, im, E->model_order, blk)) return MW_ERR_CUDA;
+  DevBuf<int> d_env_model, d_diag; DevBuf<unsigned> d_env_cost, d_env_cycles, d_env_prof; DevBuf<float4> d_sep_hint; DevBuf<MwEnvState> d_state;
+  CK(d_env_model.upload(im));
+  CK(d_env_cost.alloc(n_envs, true));
+  CK(d_env_cycles.alloc(n_envs, true));
+  // zeroed = no hint anywhere.  Never invalidated: a stale hint can only fail to reject a pair (sep_hint_test), so resets,
+  // set_state and checkpoints leave the table alone
+  CK(d_sep_hint.alloc((size_t)MW_NCONV * n_envs, true));
+  CK(d_state.alloc(n_envs, true));
+  if (E->profiling) CK(d_env_prof.alloc((size_t)MW_ENVPROF_W * n_envs, true));
+  CK(d_diag.alloc(3 * (size_t)n_envs, true));
+  E->blk = std::move(blk); E->d_env_model = std::move(d_env_model); E->d_diag = std::move(d_diag);
+  E->d_env_cost = std::move(d_env_cost); E->d_env_cycles = std::move(d_env_cycles); E->d_env_prof = std::move(d_env_prof);
+  E->d_sep_hint = std::move(d_sep_hint); E->d_state = std::move(d_state);
   E->env_model = im;
   E->n_envs = n_envs;
   E->h_faults.assign(n_envs, 0);
-  if (upload_env_blocks(E) || upload(&E->d_env_model, im)) return MW_ERR_CUDA;
-  if (E->d_env_cost) cudaFree(E->d_env_cost);
-  CK(cudaMalloc((void**)&E->d_env_cost, sizeof(unsigned) * n_envs));
-  CK(cudaMemset(E->d_env_cost, 0, sizeof(unsigned) * n_envs));
-  if (E->d_env_cycles) cudaFree(E->d_env_cycles);
-  CK(cudaMalloc((void**)&E->d_env_cycles, sizeof(unsigned) * n_envs));
-  CK(cudaMemset(E->d_env_cycles, 0, sizeof(unsigned) * n_envs));
-  // zeroed = no hint anywhere.  Never invalidated: a stale hint can only fail to reject a pair (sep_hint_test), so resets,
-  // set_state and checkpoints leave the table alone
-  if (E->d_sep_hint) cudaFree(E->d_sep_hint);
-  CK(cudaMalloc((void**)&E->d_sep_hint, sizeof(float4) * MW_NCONV * n_envs));
-  CK(cudaMemset(E->d_sep_hint, 0, sizeof(float4) * MW_NCONV * n_envs));
-  if (E->d_state) cudaFree(E->d_state);
-  CK(cudaMalloc((void**)&E->d_state, sizeof(MwEnvState) * n_envs));
-  CK(cudaMemset(E->d_state, 0, sizeof(MwEnvState) * n_envs));
-  if (E->d_env_prof) { cudaFree(E->d_env_prof); E->d_env_prof = nullptr; }
-  if (E->profiling) { CK(cudaMalloc((void**)&E->d_env_prof, sizeof(unsigned) * MW_ENVPROF_W * n_envs)); CK(cudaMemset(E->d_env_prof, 0, sizeof(unsigned) * MW_ENVPROF_W * n_envs)); }
-  if (E->d_diag) cudaFree(E->d_diag);
-  CK(cudaMalloc((void**)&E->d_diag, sizeof(int) * 3 * n_envs));
-  CK(cudaMemset(E->d_diag, 0, sizeof(int) * 3 * n_envs));
   return MW_OK;
 }
 
 int mw_build_snapshots(mw_engine* E, int n, const int* model_idx, const double* rand_vec, const double* rand_vec_pass1, const unsigned char* partial, int* ids_out) {
   if (!E || n <= 0 || !model_idx || !rand_vec || !partial) return fail(MW_ERR_ARG, "mw_build_snapshots: bad arguments");
   CK(cudaSetDevice(E->device));
-  if (E->n_snaps + n > E->snap_cap) {
-    int cap = (E->n_snaps + n) * 2;
-    MwSnapshot* p = nullptr;
-    CK(cudaMalloc((void**)&p, sizeof(MwSnapshot) * cap));
-    if (E->n_snaps) CK(cudaMemcpy(p, E->d_snaps, sizeof(MwSnapshot) * E->n_snaps, cudaMemcpyDeviceToDevice));
-    cudaFree(E->d_snaps); E->d_snaps = p; E->snap_cap = cap;
-  }
   std::vector<int> im(model_idx, model_idx + n), bm, bs, bc, perm;
   for (int v : im) if (v < 0 || v >= E->n_models) return fail(MW_ERR_ARG, "mw_build_snapshots: model index out of range");
+  if (reserve_snapshots(E, n)) return MW_ERR_CUDA;
   make_blocks(E->n_models, im, bm, bs, bc, perm);
   if (ensure_epa(E, bm.size())) return MW_ERR_CUDA;
-  int *d_bm = nullptr, *d_bs = nullptr, *d_bc = nullptr, *d_perm = nullptr; double* d_rv = nullptr; unsigned char* d_po = nullptr;
-  if (upload(&d_bm, bm) || upload(&d_bs, bs) || upload(&d_bc, bc) || upload(&d_perm, perm)) return MW_ERR_CUDA;
-  CK(cudaMalloc((void**)&d_rv, sizeof(double) * 6 * n)); CK(cudaMemcpy(d_rv, rand_vec, sizeof(double) * 6 * n, cudaMemcpyHostToDevice));
-  CK(cudaMalloc((void**)&d_po, n)); CK(cudaMemcpy(d_po, partial, n, cudaMemcpyHostToDevice));
-  double* d_rv1 = nullptr;
-  if (rand_vec_pass1) { CK(cudaMalloc((void**)&d_rv1, sizeof(double) * 6 * n)); CK(cudaMemcpy(d_rv1, rand_vec_pass1, sizeof(double) * 6 * n, cudaMemcpyHostToDevice)); }
-  k_snapshot<<<(int)bm.size(), BLOCK_THREADS, smem_bytes()>>>(E->dev(), BlockTable{d_bm, d_bs, d_bc, d_perm}, d_rv, d_rv1, d_po, E->n_snaps);
+  DevBuf<int> d_bm, d_bs, d_bc, d_perm; DevBuf<double> d_rv, d_rv1; DevBuf<unsigned char> d_po;
+  CK(d_bm.upload(bm)); CK(d_bs.upload(bs)); CK(d_bc.upload(bc)); CK(d_perm.upload(perm));
+  CK(d_rv.upload(rand_vec, 6 * (size_t)n));
+  CK(d_po.upload(partial, n));
+  if (rand_vec_pass1) CK(d_rv1.upload(rand_vec_pass1, 6 * (size_t)n));
+  k_snapshot<<<(int)bm.size(), BLOCK_THREADS, smem_bytes()>>>(E->dev(), BlockTable{d_bm.p, d_bs.p, d_bc.p, d_perm.p}, d_rv.p, d_rv1.p, d_po.p, E->n_snaps);
   CK(cudaGetLastError());
   CK(cudaDeviceSynchronize());
-  cudaFree(d_bm); cudaFree(d_bs); cudaFree(d_bc); cudaFree(d_perm); cudaFree(d_rv); cudaFree(d_rv1); cudaFree(d_po);
   if (ids_out) for (int i = 0; i < n; i++) ids_out[i] = E->n_snaps + i;
   E->n_snaps += n; E->launches++;
   return MW_OK;
@@ -969,16 +1003,10 @@ int mw_build_snapshots(mw_engine* E, int n, const int* model_idx, const double* 
 int mw_append_snapshots(mw_engine* E, int n, const void* records, int* ids_out) {
   if (!E || n <= 0 || !records) return fail(MW_ERR_ARG, "mw_append_snapshots: bad arguments");
   CK(cudaSetDevice(E->device));
-  if (E->n_snaps + n > E->snap_cap) {
-    int cap = (E->n_snaps + n) * 2;
-    MwSnapshot* p = nullptr;
-    CK(cudaMalloc((void**)&p, sizeof(MwSnapshot) * cap));
-    if (E->n_snaps) CK(cudaMemcpy(p, E->d_snaps, sizeof(MwSnapshot) * E->n_snaps, cudaMemcpyDeviceToDevice));
-    cudaFree(E->d_snaps); E->d_snaps = p; E->snap_cap = cap;
-  }
+  if (reserve_snapshots(E, n)) return MW_ERR_CUDA;
   std::vector<MwSnapshot> tmp((const MwSnapshot*)records, (const MwSnapshot*)records + n);
   for (int i = 0; i < n; i++) tmp[i].st.snapshot = (float)(E->n_snaps + i);
-  CK(cudaMemcpy(E->d_snaps + E->n_snaps, tmp.data(), sizeof(MwSnapshot) * n, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(E->d_snaps.p + E->n_snaps, tmp.data(), sizeof(MwSnapshot) * n, cudaMemcpyHostToDevice));
   if (ids_out) for (int i = 0; i < n; i++) ids_out[i] = E->n_snaps + i;
   E->n_snaps += n;
   return MW_OK;
@@ -987,28 +1015,24 @@ int mw_num_snapshots(const mw_engine* E) { return E ? E->n_snaps : 0; }
 int mw_get_snapshots(mw_engine* E, int first, int n, void* out) {
   if (!E || first < 0 || first + n > E->n_snaps) return fail(MW_ERR_ARG, "mw_get_snapshots: range");
   CK(cudaSetDevice(E->device));
-  CK(cudaMemcpy(out, E->d_snaps + first, sizeof(MwSnapshot) * n, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(out, E->d_snaps.p + first, sizeof(MwSnapshot) * n, cudaMemcpyDeviceToHost));
   return MW_OK;
 }
 
 int mw_reset(mw_engine* E, int n, const int* env_ids, const int* snapshot_ids, float* obs, int obs_stride, void* stream) {
-  if (!E || !E->d_state || n <= 0 || !snapshot_ids || !obs || obs_stride < 39) return fail(MW_ERR_ARG, "mw_reset: bad arguments");
+  if (!E || !E->d_state.p || n <= 0 || !snapshot_ids || !obs || obs_stride < 39) return fail(MW_ERR_ARG, "mw_reset: bad arguments");
   CK(cudaSetDevice(E->device));
-  k_reset<<<(n * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(E->dev(), n, env_ids, snapshot_ids, obs, obs_stride);
-  CK(cudaGetLastError());
-  E->launches++;
-  return MW_OK;
+  k_reset<<<row_blocks(n), ROW_THREADS, 0, (cudaStream_t)stream>>>(E->dev(), n, env_ids, snapshot_ids, obs, obs_stride);
+  return launched(E, 1);
 }
 
 int mw_reset_masked(mw_engine* E, const unsigned char* mask, const int* snapshot_ids, float* obs, int obs_stride, void* stream) {
-  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_reset_masked: mw_set_envs not called");
+  if (!E || !E->d_state.p) return fail(MW_ERR_STATE, "mw_reset_masked: mw_set_envs not called");
   if (!mask || !obs || obs_stride < 39) return fail(MW_ERR_ARG, "mw_reset_masked: bad arguments");
-  if (!snapshot_ids && !E->d_goal_first) return fail(MW_ERR_STATE, "mw_reset_masked: no snapshot_ids and no goal sets for the device sampler");
+  if (!snapshot_ids && !E->d_goal_first.p) return fail(MW_ERR_STATE, "mw_reset_masked: no snapshot_ids and no goal sets for the device sampler");
   CK(cudaSetDevice(E->device));
-  k_reset_masked<<<(E->n_envs * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(E->dev(), mask, snapshot_ids, obs, obs_stride);
-  CK(cudaGetLastError());
-  E->launches++;
-  return MW_OK;
+  k_reset_masked<<<row_blocks(E->n_envs), ROW_THREADS, 0, (cudaStream_t)stream>>>(E->dev(), mask, snapshot_ids, obs, obs_stride);
+  return launched(E, 1);
 }
 
 int mw_set_autoreset_mode(mw_engine* E, int mode) {
@@ -1020,76 +1044,67 @@ int mw_set_autoreset_mode(mw_engine* E, int mode) {
 
 int mw_step(mw_engine* E, const float* actions, float* obs, int obs_stride, float* reward, unsigned char* terminated, unsigned char* truncated,
             float* info, int info_stride, float* final_obs, float* final_info, const int* next_snapshot, void* stream) {
-  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_step: mw_set_envs not called");
+  if (!E || !E->d_state.p) return fail(MW_ERR_STATE, "mw_step: mw_set_envs not called");
   if (!actions || !obs || !reward || !terminated || !truncated || !info || obs_stride < 39 || info_stride < 7) return fail(MW_ERR_ARG, "mw_step: bad arguments");
-  if (!next_snapshot && !E->d_goal_first) return fail(MW_ERR_STATE, "mw_step: no next_snapshot and no goal sets for the device sampler");
+  if (!next_snapshot && !E->d_goal_first.p) return fail(MW_ERR_STATE, "mw_step: no next_snapshot and no goal sets for the device sampler");
   CK(cudaSetDevice(E->device));
+  const EnvBlocks& B = E->blk;
+  const int nb = B.n_split ? B.n_blocks_total : B.n_blocks;
   {   // launch order from the previous step's per-env cost (see k_order_*)
     int Pm = 1; while (Pm < E->n_envs && Pm < MW_SORT_MAX) Pm <<= 1;
-    const int nb = E->n_split ? E->n_blocks_total : E->n_blocks;
     int Pb = 1; while (Pb < nb && Pb < MW_SORT_MAX) Pb <<= 1;
-    k_order_envs<<<E->n_sorted_models, 1024, sizeof(unsigned long long) * Pm, (cudaStream_t)stream>>>(E->d_model_first, E->d_model_count, E->d_perm, E->d_env_cost);
-    k_order_blocks<<<1, 1024, sizeof(unsigned long long) * Pb, (cudaStream_t)stream>>>(nb, E->d_block_start, E->d_block_count, E->d_perm, E->d_env_cost, E->order_by_cycles ? E->d_env_cycles : nullptr, E->d_block_order,
-        E->n_blocks, E->n_split, E->d_split_head, E->d_split_alt, E->d_split_state, E->n_split ? E->d_block_live : nullptr, E->split_frac, E->n_sm);
+    k_order_envs<<<B.n_sorted_models, 1024, sizeof(unsigned long long) * Pm, (cudaStream_t)stream>>>(B.model_first.p, B.model_count.p, B.perm.p, E->d_env_cost.p);
+    k_order_blocks<<<1, 1024, sizeof(unsigned long long) * Pb, (cudaStream_t)stream>>>(nb, B.start.p, B.count.p, B.perm.p, E->d_env_cost.p, E->order_by_cycles ? E->d_env_cycles.p : nullptr, B.order.p,
+        B.n_blocks, B.n_split, B.split_head.p, B.split_alt.p, B.split_state.p, B.n_split ? B.live.p : nullptr, E->split_frac, E->n_sm);
   }
   auto* kern = E->autoreset_mode == MW_AUTORESET_SAME_STEP ? k_step<false> : k_step<true>;
-  kern<<<E->n_split ? E->n_blocks_total : E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->d_block_order, E->blocks(),
-      actions, obs, obs_stride, reward, terminated, truncated, info, info_stride, final_obs, final_info, next_snapshot, E->n_split ? E->d_block_live : nullptr);
-  CK(cudaGetLastError());
-  E->launches += 3; E->env_steps += (unsigned long long)E->n_envs;
+  kern<<<nb, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), B.order.p, E->blocks(),
+      actions, obs, obs_stride, reward, terminated, truncated, info, info_stride, final_obs, final_info, next_snapshot, B.n_split ? B.live.p : nullptr);
+  if (launched(E, 3)) return MW_ERR_CUDA;
+  E->env_steps += (unsigned long long)E->n_envs;
   return MW_OK;
 }
 
 int mw_evaluate(mw_engine* E, const float* actions, const float* obs, int obs_stride, float* out, void* stream) {
-  if (!E || !E->d_state || !actions || !obs || !out || obs_stride < 39) return fail(MW_ERR_ARG, "mw_evaluate: bad arguments");
+  if (!E || !E->d_state.p || !actions || !obs || !out || obs_stride < 39) return fail(MW_ERR_ARG, "mw_evaluate: bad arguments");
   CK(cudaSetDevice(E->device));
-  k_evaluate<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), actions, obs, obs_stride, out);
-  CK(cudaGetLastError());
-  E->launches++;
-  return MW_OK;
+  k_evaluate<<<E->blk.n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), actions, obs, obs_stride, out);
+  return launched(E, 1);
 }
 
 int mw_set_physics(mw_engine* E, const unsigned char* mask, const double* qpos, const double* qvel, void* stream) {
-  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_set_physics: mw_set_envs not called");
+  if (!E || !E->d_state.p) return fail(MW_ERR_STATE, "mw_set_physics: mw_set_envs not called");
   if (!mask || !qpos || !qvel) return fail(MW_ERR_ARG, "mw_set_physics: bad arguments");
   CK(cudaSetDevice(E->device));
-  k_set_physics<<<(E->n_envs * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(E->dev(), E->d_env_model, mask, qpos, qvel);
-  CK(cudaGetLastError());
-  E->launches++;
-  return MW_OK;
+  k_set_physics<<<row_blocks(E->n_envs), ROW_THREADS, 0, (cudaStream_t)stream>>>(E->dev(), E->d_env_model.p, mask, qpos, qvel);
+  return launched(E, 1);
 }
 
 int mw_get_physics(mw_engine* E, double* qpos, double* qvel, void* stream) {
-  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_get_physics: mw_set_envs not called");
+  if (!E || !E->d_state.p) return fail(MW_ERR_STATE, "mw_get_physics: mw_set_envs not called");
   if (!qpos || !qvel) return fail(MW_ERR_ARG, "mw_get_physics: bad arguments");
   CK(cudaSetDevice(E->device));
-  k_get_physics<<<(E->n_envs * 32 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(E->dev(), E->d_env_model, qpos, qvel);
-  CK(cudaGetLastError());
-  E->launches++;
-  return MW_OK;
+  k_get_physics<<<row_blocks(E->n_envs), ROW_THREADS, 0, (cudaStream_t)stream>>>(E->dev(), E->d_env_model.p, qpos, qvel);
+  return launched(E, 1);
 }
 
 int mw_observe(mw_engine* E, const unsigned char* mask, float* obs, int obs_stride, void* stream) {
-  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_observe: mw_set_envs not called");
+  if (!E || !E->d_state.p) return fail(MW_ERR_STATE, "mw_observe: mw_set_envs not called");
   if (!mask || !obs || obs_stride < 39) return fail(MW_ERR_ARG, "mw_observe: bad arguments");
   CK(cudaSetDevice(E->device));
-  k_observe<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), mask, obs, obs_stride);
-  CK(cudaGetLastError());
-  E->launches++;
-  return MW_OK;
+  k_observe<<<E->blk.n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), mask, obs, obs_stride);
+  return launched(E, 1);
 }
 
 int mw_query(mw_engine* E, const unsigned char* mask, float* frame, const void* frames, int n_frames, double* pose,
              const int* touch_geom, unsigned char* touching, void* stream) {
-  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_query: mw_set_envs not called");
+  if (!E || !E->d_state.p) return fail(MW_ERR_STATE, "mw_query: mw_set_envs not called");
   if (!mask || n_frames < 0 || (pose && (!frames || n_frames == 0)) || (!touching) != (!touch_geom))
     return fail(MW_ERR_ARG, "mw_query: bad arguments");
   if (!frame && !pose && !touching) return MW_OK;
   CK(cudaSetDevice(E->device));
-  k_query<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), mask, frame, (const MwQueryFrame*)frames, pose ? n_frames : 0, pose, touch_geom, touching);
-  CK(cudaGetLastError());
-  E->launches++;
-  return MW_OK;
+  k_query<<<E->blk.n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), mask, frame, (const MwQueryFrame*)frames, pose ? n_frames : 0, pose, touch_geom, touching);
+  return launched(E, 1);
 }
 
 int mw_expert_actions(const int* task_ids, const float* obs, int obs_stride, int n, float* actions, void* stream) {
@@ -1101,12 +1116,13 @@ int mw_expert_actions(const int* task_ids, const float* obs, int obs_stride, int
 }
 
 int mw_get_faults(mw_engine* E, int* out) {
-  if (!E || !out || !E->d_diag) return fail(MW_ERR_ARG, "mw_get_faults");
+  if (!E || !out || !E->d_diag.p) return fail(MW_ERR_ARG, "mw_get_faults");
   CK(cudaSetDevice(E->device));
-  std::vector<int> diag(3 * (size_t)E->n_envs);
-  CK(cudaMemcpy(diag.data(), E->d_diag, sizeof(int) * diag.size(), cudaMemcpyDeviceToHost));
-  for (int i = 0; i < E->n_envs; i++) { out[i] = E->h_faults[i] | diag[3 * i + 2]; E->h_faults[i] = 0; diag[3 * i + 2] = 0; }
-  CK(cudaMemcpy(E->d_diag, diag.data(), sizeof(int) * diag.size(), cudaMemcpyHostToDevice));
+  std::vector<int> diag;
+  if (read_diag(E, diag)) return MW_ERR_CUDA;
+  for (int i = 0; i < E->n_envs; i++) { out[i] = E->h_faults[i] | diag[3 * i + 2]; diag[3 * i + 2] = 0; }
+  CK(cudaMemcpy(E->d_diag.p, diag.data(), sizeof(int) * diag.size(), cudaMemcpyHostToDevice));
+  E->h_faults.assign(E->n_envs, 0);
   return MW_OK;
 }
 
@@ -1120,45 +1136,44 @@ int mw_set_goal_sets(mw_engine* E, const int* first, const int* count) {
   CK(cudaSetDevice(E->device));
   std::vector<int> f(first, first + E->n_envs), c(count, count + E->n_envs);
   for (int i = 0; i < E->n_envs; i++) if (c[i] <= 0 || f[i] < 0 || f[i] + c[i] > E->n_snaps) return fail(MW_ERR_ARG, "mw_set_goal_sets: range outside the snapshot table");
-  if (upload(&E->d_goal_first, f) || upload(&E->d_goal_count, c)) return MW_ERR_CUDA;
+  DevBuf<int> d_first, d_count;
+  CK(d_first.upload(f)); CK(d_count.upload(c));
+  E->d_goal_first = std::move(d_first); E->d_goal_count = std::move(d_count);
   return MW_OK;
 }
 int mw_get_state(mw_engine* E, void* out) {
-  if (!E || !E->d_state || !out) return fail(MW_ERR_ARG, "mw_get_state");
+  if (!E || !E->d_state.p || !out) return fail(MW_ERR_ARG, "mw_get_state");
   CK(cudaSetDevice(E->device));
-  CK(cudaMemcpy(out, E->d_state, sizeof(MwEnvState) * E->n_envs, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(out, E->d_state.p, sizeof(MwEnvState) * E->n_envs, cudaMemcpyDeviceToHost));
   return MW_OK;
 }
 int mw_set_state(mw_engine* E, const void* in) {
-  if (!E || !E->d_state || !in) return fail(MW_ERR_ARG, "mw_set_state");
+  if (!E || !E->d_state.p || !in) return fail(MW_ERR_ARG, "mw_set_state");
   CK(cudaSetDevice(E->device));
-  CK(cudaMemcpy(E->d_state, in, sizeof(MwEnvState) * E->n_envs, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(E->d_state.p, in, sizeof(MwEnvState) * E->n_envs, cudaMemcpyHostToDevice));
   return MW_OK;
 }
 int mw_debug_substeps(mw_engine* E, int nstep, const float* ctrl2, void* stream) {
-  if (!E || !E->d_state || nstep < 0 || !ctrl2) return fail(MW_ERR_ARG, "mw_debug_substeps");
+  if (!E || !E->d_state.p || nstep < 0 || !ctrl2) return fail(MW_ERR_ARG, "mw_debug_substeps");
   CK(cudaSetDevice(E->device));
-  k_substeps<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), nstep, ctrl2[0], ctrl2[1], nullptr);
-  CK(cudaGetLastError());
-  E->launches++;
-  return MW_OK;
+  k_substeps<<<E->blk.n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), nstep, ctrl2[0], ctrl2[1], nullptr);
+  return launched(E, 1);
 }
 int mw_debug_forward(mw_engine* E, const float* ctrl2, float* dump_dev, void* stream) {
-  if (!E || !E->d_state || !ctrl2 || !dump_dev) return fail(MW_ERR_ARG, "mw_debug_forward");
+  if (!E || !E->d_state.p || !ctrl2 || !dump_dev) return fail(MW_ERR_ARG, "mw_debug_forward");
   CK(cudaSetDevice(E->device));
-  k_substeps<<<E->n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), 0, ctrl2[0], ctrl2[1], dump_dev);
-  CK(cudaGetLastError());
-  return MW_OK;
+  k_substeps<<<E->blk.n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), 0, ctrl2[0], ctrl2[1], dump_dev);
+  return launched(E, 0);   // a debug dump: not counted
 }
 int mw_debug_dump_floats(void) { return MW_MAXCON * 12 + MW_MAXDOF + 4; }
 int mw_get_counters(mw_engine* E, unsigned long long* out5) {
   if (!E || !out5) return fail(MW_ERR_ARG, "mw_get_counters");
   CK(cudaSetDevice(E->device));
-  std::vector<int> diag(3 * (size_t)(E->n_envs > 0 ? E->n_envs : 0));
+  std::vector<int> diag;
+  if (read_diag(E, diag)) return MW_ERR_CUDA;
   if (E->n_envs) {
-    CK(cudaMemcpy(diag.data(), E->d_diag, sizeof(int) * diag.size(), cudaMemcpyDeviceToHost));
+    CK(cudaMemset(E->d_diag.p, 0, sizeof(int) * diag.size()));
     for (int i = 0; i < E->n_envs; i++) { E->h_faults[i] |= diag[3 * i + 2]; }
-    CK(cudaMemset(E->d_diag, 0, sizeof(int) * diag.size()));
   }
   unsigned long long dropped = 0, iters = 0;
   for (int i = 0; i < E->n_envs; i++) { dropped += diag[3 * i]; iters += diag[3 * i + 1]; }
@@ -1168,47 +1183,50 @@ int mw_get_counters(mw_engine* E, unsigned long long* out5) {
 }
 
 int mw_rebalance(mw_engine* E) {
-  if (!E || !E->d_state) return fail(MW_ERR_STATE, "mw_rebalance: mw_set_envs not called");
+  if (!E || !E->d_state.p) return fail(MW_ERR_STATE, "mw_rebalance: mw_set_envs not called");
   CK(cudaSetDevice(E->device));
   CK(cudaDeviceSynchronize());
   std::vector<unsigned long long> mc(2 * (size_t)E->n_models);
-  CK(cudaMemcpy(mc.data(), E->d_model_cycles, sizeof(unsigned long long) * mc.size(), cudaMemcpyDeviceToHost));
-  CK(cudaMemset(E->d_model_cycles, 0, sizeof(unsigned long long) * mc.size()));
+  CK(cudaMemcpy(mc.data(), E->d_model_cycles.p, sizeof(unsigned long long) * mc.size(), cudaMemcpyDeviceToHost));
   std::vector<std::pair<double, int>> cost;
   for (int i = 0; i < E->n_models; i++) cost.push_back({mc[2 * i + 1] ? (double)mc[2 * i] / (double)mc[2 * i + 1] : 0.0, i});
   std::stable_sort(cost.begin(), cost.end(), [](const std::pair<double, int>& a, const std::pair<double, int>& b) { return a.first > b.first; });
-  E->model_order.clear();
-  for (auto& c : cost) E->model_order.push_back(c.second);
-  if (upload_env_blocks(E)) return MW_ERR_CUDA;
+  std::vector<int> order;
+  for (auto& c : cost) order.push_back(c.second);
+  EnvBlocks blk;
+  if (upload_env_blocks(E, E->env_model, order, blk)) return MW_ERR_CUDA;
+  CK(cudaMemset(E->d_model_cycles.p, 0, sizeof(unsigned long long) * mc.size()));
+  E->blk = std::move(blk);
+  E->model_order = order;
   return MW_OK;
 }
 
 int mw_set_profiling(mw_engine* E, int on) {
   if (!E) return fail(MW_ERR_ARG, "mw_set_profiling");
   CK(cudaSetDevice(E->device));
+  if (on && E->n_envs && !E->d_env_prof.p) CK(E->d_env_prof.alloc((size_t)MW_ENVPROF_W * E->n_envs, true));
   E->profiling = on ? 1 : 0;
-  if (on && E->n_envs && !E->d_env_prof) { CK(cudaMalloc((void**)&E->d_env_prof, sizeof(unsigned) * MW_ENVPROF_W * E->n_envs)); CK(cudaMemset(E->d_env_prof, 0, sizeof(unsigned) * MW_ENVPROF_W * E->n_envs)); }
   return MW_OK;
 }
 int mw_get_env_profile(mw_engine* E, unsigned* out) {
-  if (!E || !out || !E->d_env_prof) return fail(MW_ERR_STATE, "mw_get_env_profile: profiling is off (mw_set_profiling)");
+  if (!E || !out || !E->d_env_prof.p) return fail(MW_ERR_STATE, "mw_get_env_profile: profiling is off (mw_set_profiling)");
   CK(cudaSetDevice(E->device));
-  CK(cudaMemcpy(out, E->d_env_prof, sizeof(unsigned) * MW_ENVPROF_W * E->n_envs, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(out, E->d_env_prof.p, sizeof(unsigned) * MW_ENVPROF_W * E->n_envs, cudaMemcpyDeviceToHost));
   return MW_OK;
 }
 
 int mw_get_env_cost(mw_engine* E, unsigned* out) {
-  if (!E || !out || !E->d_env_cost) return fail(MW_ERR_ARG, "mw_get_env_cost");
+  if (!E || !out || !E->d_env_cost.p) return fail(MW_ERR_ARG, "mw_get_env_cost");
   CK(cudaSetDevice(E->device));
-  CK(cudaMemcpy(out, E->d_env_cost, sizeof(unsigned) * E->n_envs, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(out, E->d_env_cost.p, sizeof(unsigned) * E->n_envs, cudaMemcpyDeviceToHost));
   return MW_OK;
 }
 
 int mw_get_profile(mw_engine* E, unsigned long long* out15) {
   if (!E || !out15) return fail(MW_ERR_ARG, "mw_get_profile");
   CK(cudaSetDevice(E->device));
-  CK(cudaMemcpy(out15, E->d_prof, sizeof(unsigned long long) * 15, cudaMemcpyDeviceToHost));
-  CK(cudaMemset(E->d_prof, 0, sizeof(unsigned long long) * 16));
+  CK(cudaMemcpy(out15, E->d_prof.p, sizeof(unsigned long long) * 15, cudaMemcpyDeviceToHost));
+  CK(cudaMemset(E->d_prof.p, 0, sizeof(unsigned long long) * 16));
   return MW_OK;
 }
 

@@ -756,3 +756,72 @@ def test_head_split_is_pure_scheduling(torch_cuda, tmp_path):
         outs.append(json.load(open(out)))
     a, b = outs
     assert a["steps"] == b["steps"] and a["state"] == b["state"] and a["dropped"] == b["dropped"] == 0
+
+
+def test_env_table_replacement_failed_calls_and_rebalance_keep_results(torch_cuda):
+    """The host paths that rebuild an engine's tables.  (a) `set_envs` on an engine that already holds snapshots and envs,
+    to a larger and then a smaller set, replaces every per-env buffer and the CTA table: each set steps bitwise as on a
+    fresh engine.  (b) `set_envs` / `build_snapshots` with a model index out of range fail and change nothing: snapshot
+    count and state records stay, and the engine steps on bitwise as one that never made those calls.  (c) `rebalance`
+    re-sorts the CTA launch order by measured model cost, which is pure scheduling: outputs stay bitwise equal."""
+    from metaworld_b200 import benchmarks as B
+    from metaworld_b200.engine import Engine, EngineError, lib
+    t = torch_cuda
+    tasks = ["reach-v3", "push-v3"]
+    rv = [g.unpack()["rand_vec"] for k in tasks for g in B.make_tasks([k], False, seed=3, n_goals=2)]
+
+    def engine(env_model, profiling=False):
+        e = Engine(tasks)
+        assert list(e.build_snapshots([0, 0, 1, 1], rv, [0] * 4)) == [0, 1, 2, 3]
+        e.set_options(500, False, 0)
+        e.set_profiling(profiling)
+        e.set_envs(env_model)
+        return e
+
+    def start(e, env_model):
+        """Resets every env from a snapshot of its model; returns step(k): the bytes of k steps' outputs + state records."""
+        n, d = len(env_model), e.device
+        sid = t.tensor([2 * m + i % 2 for i, m in enumerate(env_model)], dtype=t.int32, device=d)
+        obs, fobs = t.zeros(n, 39, device=d), t.zeros(n, 39, device=d)
+        rew, info, finfo = t.zeros(n, device=d), t.zeros(n, 7, device=d), t.zeros(n, 8, device=d)
+        term, trunc = t.zeros(n, dtype=t.uint8, device=d), t.zeros(n, dtype=t.uint8, device=d)
+        e.reset(sid, obs)
+        rng = np.random.default_rng(n)
+
+        def step(k):
+            out = [obs.cpu().numpy().tobytes()]
+            for _ in range(k):
+                a = t.tensor(rng.uniform(-1, 1, (n, 4)).astype(np.float32), device=d)
+                e.step(a, obs, rew, term, trunc, info, fobs, finfo, sid)
+                out += [x.cpu().numpy().tobytes() for x in (obs, rew, info, term, trunc, fobs, finfo)]
+            return out + [e.get_state().tobytes()]
+        return step
+
+    sets = ([1, 0, 1], [i % 3 // 2 for i in range(24)], [0, 1])
+    a = engine(sets[0])
+    for env_model in sets:
+        a.set_envs(env_model)
+        b = engine(env_model)
+        assert start(a, env_model)(6) == start(b, env_model)(6)
+        b.close()
+
+    env_model = sets[1]
+    a.set_envs(env_model)
+    b = engine(env_model)
+    sa, sb = start(a, env_model), start(b, env_model)
+    assert sa(3) == sb(3)
+    n_snaps, st = lib().mw_num_snapshots(a.h), a.get_state().tobytes()
+    with pytest.raises(EngineError):
+        a.set_envs([0, 2])
+    with pytest.raises(EngineError):
+        a.build_snapshots([0, 2], rv[:2], [0, 0], precise=False)
+    assert lib().mw_num_snapshots(a.h) == n_snaps and a.get_state().tobytes() == st
+    assert sa(5) == sb(5)
+    a.close(); b.close()
+
+    a, b = engine(env_model, profiling=True), engine(env_model, profiling=True)
+    sa, sb = start(a, env_model), start(b, env_model)
+    assert sa(4) == sb(4)
+    a.rebalance()
+    assert sa(6) == sb(6)
+    a.close(); b.close()

@@ -128,6 +128,42 @@ def test_cabi_exports_every_declared_symbol(built):
             engine.Engine(["reach-v3"])
 
 
+def test_cabi_rejects_a_null_engine(built):
+    """Every entry point that takes an engine answers NULL with its own status and message and touches no device: a
+    caller that lost its handle gets an error it can act on, never a crash."""
+    from metaworld_b200 import engine
+    buf = np.zeros(1 << 16, dtype=np.uint8)
+    p = buf.ctypes.data                     # well-formed host storage for every pointer argument
+    bad = "{}: bad arguments"
+    not_set = "{}: mw_set_envs not called"
+    ARG, STATE = -2, -3
+    calls = {
+        "mw_set_envs": ((1, p), ARG, bad), "mw_build_snapshots": ((1, p, p, None, p, p), ARG, bad),
+        "mw_append_snapshots": ((1, p, p), ARG, bad), "mw_reset": ((1, None, p, p, 39, None), ARG, bad),
+        "mw_evaluate": ((p, p, 39, p, None), ARG, bad), "mw_set_options": ((500, 0, 0), ARG, bad),
+        "mw_set_goal_sets": ((p, p), ARG, bad),
+        "mw_reset_masked": ((p, p, p, 39, None), STATE, not_set),
+        "mw_step": ((p, p, 39, p, p, p, p, 9, p, p, p, None), STATE, not_set),
+        "mw_set_physics": ((p, p, p, None), STATE, not_set), "mw_get_physics": ((p, p, None), STATE, not_set),
+        "mw_observe": ((p, p, 39, None), STATE, not_set), "mw_query": ((p, p, p, 1, p, p, p, None), STATE, not_set),
+        "mw_rebalance": ((), STATE, not_set),
+        "mw_get_faults": ((p,), ARG, "{}"), "mw_get_state": ((p,), ARG, "{}"), "mw_set_state": ((p,), ARG, "{}"),
+        "mw_debug_substeps": ((1, p, None), ARG, "{}"), "mw_debug_forward": ((p, p, None), ARG, "{}"),
+        "mw_get_counters": ((p,), ARG, "{}"), "mw_set_profiling": ((1,), ARG, "{}"), "mw_get_profile": ((p,), ARG, "{}"),
+        "mw_get_env_cost": ((p,), ARG, "{}"),
+        "mw_get_snapshots": ((0, 1, p), ARG, "{}: range"),
+        "mw_set_autoreset_mode": ((0,), ARG, "{}: mode must be MW_AUTORESET_SAME_STEP, _NEXT_STEP or _DISABLED"),
+        "mw_get_env_profile": ((p,), STATE, "{}: profiling is off (mw_set_profiling)"),
+    }
+    for so in ("libmwb200.so", "libmwb200_f64.so"):
+        lib = engine._load(os.path.join(ROOT, "metaworld_b200", so))
+        for name, (args, code, msg) in calls.items():
+            assert getattr(lib, name)(None, *args) == code, (so, name)
+            assert lib.mw_last_error().decode() == msg.format(name), (so, name)
+        assert lib.mw_num_snapshots(None) == 0
+        lib.mw_destroy(None)
+
+
 def test_product_does_not_import_oracle():
     """The oracle is test infrastructure: nothing under metaworld_b200/ may reference it."""
     for dp, _, fs in os.walk(os.path.join(ROOT, "metaworld_b200")):
