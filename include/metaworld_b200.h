@@ -200,8 +200,9 @@ int mw_get_env_profile(mw_engine*, unsigned* out /*host [n_envs*20]*/);
  * [4] bias forces + unconstrained solve, [5] constraint solver, [6] integration + glue, [7] obs / reward / autoreset,
  * [8] whole step incl. [12]; events: [9] GJK/EPA pair calls, [10] EPA expansions, [11] GJK iterations; [12] cycles spent
  * waiting for the CTA's other warps at phase boundaries (not part of [0]..[7]); [13] GJK/EPA pairs tested against their
- * separating-axis hint, [14] of those, pairs the hint proved apart (no GJK/EPA run; [2] and [9] include them) */
-int mw_get_profile(mw_engine*, unsigned long long* out15);
+ * separating-axis hint, [14] of those, pairs the hint proved apart (no GJK/EPA run; [2] and [9] include them); [15] cycles
+ * of the kinematics alone (part of [0]; every pass, the kinematics-only sixth pass included) */
+int mw_get_profile(mw_engine*, unsigned long long* out16);
 /* solver work of each environment's most recent step (host array of n_envs): the estimate, from Newton iterations weighted
  * by the constraint rows they touch, that orders a model's environments for the next launch (costliest first)       */
 int mw_get_env_cost(mw_engine*, unsigned* out);

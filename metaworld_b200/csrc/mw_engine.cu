@@ -292,7 +292,7 @@ k_step(EngineDev e, const int* __restrict__ block_order, BlockTable bt, const fl
   }
   SYNCW();
   if (e.prof) {     // profiling runs only (mw_set_profiling): summed phase counters, per-model cost, per-env record
-    if (lane < 15) atomicAdd(e.prof + lane, (unsigned long long)w->prof[lane]);
+    if (lane < 16) atomicAdd(e.prof + lane, (unsigned long long)w->prof[lane]);
     if (lane == 0 && e.model_cycles) { atomicAdd(e.model_cycles + 2 * mi, (unsigned long long)w->prof[8]); atomicAdd(e.model_cycles + 2 * mi + 1, 1ull); }
     if (e.env_prof) {
       if (lane < 13) e.env_prof[MW_ENVPROF_W * env + lane] = (unsigned)(w->prof[lane] > 0xFFFFFFFFll ? 0xFFFFFFFFll : w->prof[lane]);
@@ -898,8 +898,8 @@ int mw_sizeof_snapshot(void) { return (int)sizeof(MwSnapshot); }
 const char* mw_last_error(void) { return g_err.c_str(); }
 const char* mw_build_info(void) {
   static char buf[256];
-  snprintf(buf, sizeof(buf), "real=%s maxcon=%d(shared %d) maxefc=%d(shared %d) warps_per_block=%d smem_per_block=%zu", sizeof(real) == 4 ? "float" : "double",
-           MW_MAXCON, MW_SMCON, MW_MAXEFC, MW_SMEFC, WARPS_PER_BLOCK, smem_bytes());
+  snprintf(buf, sizeof(buf), "real=%s maxcon=%d(shared %d) maxefc=%d(shared %d) warps_per_block=%d smem_per_block=%zu%s", sizeof(real) == 4 ? "float" : "double",
+           MW_MAXCON, MW_SMCON, MW_MAXEFC, MW_SMEFC, WARPS_PER_BLOCK, smem_bytes(), MW_LINKS_INFO);
   return buf;
 }
 
@@ -1222,10 +1222,10 @@ int mw_get_env_cost(mw_engine* E, unsigned* out) {
   return MW_OK;
 }
 
-int mw_get_profile(mw_engine* E, unsigned long long* out15) {
-  if (!E || !out15) return fail(MW_ERR_ARG, "mw_get_profile");
+int mw_get_profile(mw_engine* E, unsigned long long* out16) {
+  if (!E || !out16) return fail(MW_ERR_ARG, "mw_get_profile");
   CK(cudaSetDevice(E->device));
-  CK(cudaMemcpy(out15, E->d_prof.p, sizeof(unsigned long long) * 15, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(out16, E->d_prof.p, sizeof(unsigned long long) * 16, cudaMemcpyDeviceToHost));
   CK(cudaMemset(E->d_prof.p, 0, sizeof(unsigned long long) * 16));
   return MW_OK;
 }

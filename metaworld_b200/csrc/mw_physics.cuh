@@ -66,7 +66,8 @@ struct WarpScratch {
   real ctrl[2], mocap_pos[3], mocap_quat[4], shift[3];
   real qfrc_smooth[MW_MAXDOF], qacc_smooth[MW_MAXDOF], qfrc_con[MW_MAXDOF], qacc[MW_MAXDOF];
   real vMa[MW_MAXDOF], vSearch[MW_MAXDOF], vMs[MW_MAXDOF], vTmp[MW_MAXDOF];
-  real M[MW_MAXDOF * NVP], H[MW_MAXDOF * NVP];
+  real M[MW_MAXDOF * NVP];
+  alignas(8) real H[MW_MAXDOF * NVP];   // also the links' float64 matrices from mw_kinematics to mw_collide (mw_lmatd)
   alignas(16) real U[MW_UWORDS];
   EpaWs* epa;               // this warp's GJK/EPA polytope workspace (global memory, see mw_engine.cu)
   WarpSpill* sp;            // overflow storage for contacts >= MW_SMCON / rows >= MW_SMEFC (global memory)
@@ -81,7 +82,8 @@ struct WarpScratch {
   int fault;                // MW_FAULT_* bits raised by the task code during this step (lane 0)
   int prof_on;              // phase timers enabled (mw_set_profiling)
   long long prof[16];       // cycle / event counters of this step (mw_get_profile order; [12] = cycles spent waiting in PHASE_SYNC,
-                            // [13] / [14] = convex pairs tested against / rejected by their separating-axis hint; lane 0 only)
+                            // [13] / [14] = convex pairs tested against / rejected by their separating-axis hint, [15] = cycles of
+                            // mw_kinematics alone, a part of [0]; lane 0 only)
 };
 
 struct WarpSpill {
@@ -101,14 +103,106 @@ DEV Contact* mw_con(const WarpScratch* w, int c) { return c < MW_SMCON ? (Contac
 #define SYNCW() __syncwarp()
 // cycle counter that the compiler may not move across barriers / memory operations (plain clock64() was hoisted above
 // __syncthreads(), which booked every barrier wait on the phase that follows it)
+#ifndef MW_HOST_EMU
 DEV long long mw_clock() { long long t; asm volatile("mov.u64 %0, %%clock64;" : "=l"(t) :: "memory"); return t; }
+#else
+DEV long long mw_clock() { return 0; }   // tests/kinlanes compiles this header for the host
+#endif
 // Reading the clock is not free (ncu: 5.7 % of all stall samples sat on the ~80 reads per env step), so the phase timers
 // only run while profiling is switched on (mw_set_profiling); MW_CLK(w) is 0 otherwise.
 #define MW_CLK(w) ((w)->prof_on ? mw_clock() : 0ll)
 #define QSET(w, i, v) { (w)->qposd[i] = (double)(v); (w)->qpos[i] = (real)(w)->qposd[i]; }   /* write a generalized position */
 
 // ------------------------------------------------------------------ kinematics  [MuJoCo mj_kinematics]
-// Sequential over the (short) link chain; every lane computes the same values, lane 0 stores.
+// World rotation matrices of the links in float64, left in w->H by mw_kinematics for mw_collide's geom poses.  H holds
+// nothing else between the start of a pass and mw_rne_bias.
+static_assert(sizeof(((WarpScratch*)0)->H) >= sizeof(double) * 9 * MW_MAXLINK, "w->H too small for the links' float64 matrices");
+DEV double* mw_lmatd(const WarpScratch* w, int l) { return (double*)w->H + 9 * l; }
+#ifndef MW_SERIAL_LINKS
+#define MW_LINKS_INFO ""
+// One link per lane.  What a link does not owe its parent comes first, in all lanes at once: the sincos of its hinge
+// angle, and for a free joint the whole pose.  The rest is a chain along the tree's
+// depth: level by level, the lanes whose link sits at that depth pose it from the parent's stored pose and store their
+// own.  Every expression is the one of the link-by-link form below with the same operands in the same order, and the build
+// has no multiply-add contraction, so the results are the same bits (tests/test_kinematics_lanes.py).  In particular the
+// parent's matrix read from w->H is quat2mat of the parent's stored quaternion, which is what that form computes or
+// carries in registers.
+DEV void mw_store_link(WarpScratch* w, int l, const double* pos, const double* quat, const double* R) {
+  double* Rd = mw_lmatd(w, l);
+  for (int i = 0; i < 3; i++) { w->lposd[l][i] = pos[i]; w->lpos[l][i] = (real)pos[i]; }
+  for (int i = 0; i < 4; i++) { w->lquatd[l][i] = quat[i]; w->lquat[l][i] = (real)quat[i]; }
+  for (int i = 0; i < 9; i++) { Rd[i] = R[i]; w->lmat[l][i] = (real)R[i]; }
+}
+__device__ __noinline__ void mw_kinematics(const MwModel* __restrict__ m, WarpScratch* w, int lane) {
+  const int l = lane;
+  int depth = -1, p = -1, jt = JT_HINGE, da = 0;      // depth -1: no link in this lane, or a free joint (posed below)
+  double qr[4], q = 0;                                // hinge: rotation about the joint axis; slide: displacement
+  if (l < m->nlink) {
+    jt = m->link_jtype[l]; da = m->link_dadr[l];
+    const int qa = m->link_qadr[l];
+    if (jt == JT_FREE) {
+      double pos[3], quat[4] = {w->qposd[qa + 3], w->qposd[qa + 4], w->qposd[qa + 5], w->qposd[qa + 6]}, R[9];
+      quat_normalize(quat);
+      for (int i = 0; i < 3; i++) pos[i] = w->qposd[qa + i];
+      quat2mat(R, quat);
+      for (int i = 0; i < 4; i++) QSET(w, qa + 3 + i, quat[i]);
+      for (int i = 0; i < 3; i++) {
+        for (int k = 0; k < 3; k++) { w->daxis[da + i][k] = (i == k); w->danchor[da + i][k] = (real)pos[k]; }
+        w->daxis[da + 3 + i][0] = (real)R[i]; w->daxis[da + 3 + i][1] = (real)R[3 + i]; w->daxis[da + 3 + i][2] = (real)R[6 + i];
+        for (int k = 0; k < 3; k++) w->danchor[da + 3 + i][k] = (real)pos[k];
+      }
+      mw_store_link(w, l, pos, quat, R);
+    } else {
+      depth = m->link_depth[l]; p = m->link_parent[l];
+      q = w->qposd[qa] - m->qpos0d[qa];
+      if (jt != JT_SLIDE) {
+        double jax[3] = {m->link_jaxis[l][0], m->link_jaxis[l][1], m->link_jaxis[l][2]};
+        quat_axisangle(qr, jax, q);
+      }
+    }
+  }
+  const int nd = m->ndepth;
+  for (int d = 0; d < nd; d++) {
+    if (depth == d) {
+      double pos[3], quat[4], R[9], axis[3], anchor[3], t[3];
+      double lp[3] = {m->link_pos[l][0], m->link_pos[l][1], m->link_pos[l][2]};
+      double lq[4] = {m->link_quat[l][0], m->link_quat[l][1], m->link_quat[l][2], m->link_quat[l][3]};
+      double jax[3] = {m->link_jaxis[l][0], m->link_jaxis[l][1], m->link_jaxis[l][2]};
+      double jp[3] = {m->link_jpos[l][0], m->link_jpos[l][1], m->link_jpos[l][2]};
+      if (p < 0) {
+        if (m->link_shift[l]) { for (int i = 0; i < 3; i++) pos[i] = lp[i] + (double)w->shift[i]; }
+        else { for (int i = 0; i < 3; i++) pos[i] = lp[i]; }
+        for (int i = 0; i < 4; i++) quat[i] = lq[i];
+      } else {
+        mat_mulvec(t, mw_lmatd(w, p), lp); v3add(pos, w->lposd[p], t);
+        quat_mul(quat, w->lquatd[p], lq);
+      }
+      // joint axis and anchor in the frame the body has before its own joint moves it (a product of unit quaternions:
+      // like mj_kinematics, no normalisation before the end of the body)
+      quat2mat(R, quat);
+      mat_mulvec(axis, R, jax);
+      mat_mulvec(t, R, jp); v3add(anchor, pos, t);
+      if (jt == JT_SLIDE) {
+        v3addscl(pos, pos, axis, q);
+        quat_normalize(quat); quat2mat(R, quat);
+      } else {
+        double qn[4];
+        quat_mul(qn, quat, qr);
+        for (int i = 0; i < 4; i++) quat[i] = qn[i];
+        quat_normalize(quat);
+        quat2mat(R, quat);
+        mat_mulvec(t, R, jp); v3sub(pos, anchor, t);
+      }
+      for (int k = 0; k < 3; k++) { w->daxis[da][k] = (real)axis[k]; w->danchor[da][k] = (real)anchor[k]; }
+      mw_store_link(w, l, pos, quat, R);
+    }
+    SYNCW();
+  }
+}
+#else
+#define MW_LINKS_INFO " serial links"
+// The link-by-link form (-DMW_SERIAL_LINKS: the A arm of scripts/gpu_kin_ab.py and the reference of the bitwise tests, not
+// a supported configuration).  Sequential over the links; every lane computes the same values, lane 0 stores.
 __device__ __noinline__ void mw_kinematics(const MwModel* __restrict__ m, WarpScratch* w, int lane) {
   const int nl = m->nlink;
   double quat[4], R[9];          // orientation of the link in work; at the top of an iteration: of the previous link
@@ -176,6 +270,7 @@ __device__ __noinline__ void mw_kinematics(const MwModel* __restrict__ m, WarpSc
     SYNCW();
   }
 }
+#endif
 
 // world pose of a frame / geom attached to link l (or to the world, optionally riding on the shift)
 DEV void mw_attach(const WarpScratch* w, int link, int shift, const float* lp, real* pos) {
@@ -370,62 +465,93 @@ DEV void cross_motion(real* r, const real* v, const real* s) {
   v3cross(a, v, s); v3cross(b, v, s + 3); v3cross(c, v + 3, s);
   r[0] = a[0]; r[1] = a[1]; r[2] = a[2]; r[3] = b[0] + c[0]; r[4] = b[1] + c[1]; r[5] = b[2] + c[2];
 }
+// spatial velocity / acceleration of link l from its parent's (in v, a on entry): the joint's own dofs added in dof order
+DEV void mw_rne_joint(const MwModel* __restrict__ m, const WarpScratch* w, int l, real* v, real* a) {
+  int jt = m->link_jtype[l], da = m->link_dadr[l];
+  if (jt == JT_FREE) {
+    real vb[6];
+    for (int i = 0; i < 3; i++) {   // world-fixed translation axes
+      real S[6] = {0, 0, 0, w->daxis[da + i][0], w->daxis[da + i][1], w->daxis[da + i][2]}, Sd[6];
+      cross_motion(Sd, v, S);
+      real qd = w->qvel[da + i];
+      for (int c = 0; c < 6; c++) { a[c] += Sd[c] * qd; }
+      for (int c = 0; c < 6; c++) v[c] += S[c] * qd;
+    }
+    for (int c = 0; c < 6; c++) vb[c] = v[c];
+    for (int i = 3; i < 6; i++) {   // body-fixed rotation axes: all three see the same velocity
+      real S[6], Sd[6];
+      for (int k = 0; k < 3; k++) S[k] = w->daxis[da + i][k];
+      v3cross(S + 3, w->danchor[da + i], w->daxis[da + i]);
+      cross_motion(Sd, vb, S);
+      real qd = w->qvel[da + i];
+      for (int c = 0; c < 6; c++) { a[c] += Sd[c] * qd; v[c] += S[c] * qd; }
+    }
+  } else {
+    real S[6], Sd[6];
+    if (jt == JT_HINGE) { for (int k = 0; k < 3; k++) S[k] = w->daxis[da][k]; v3cross(S + 3, w->danchor[da], w->daxis[da]); }
+    else { S[0] = S[1] = S[2] = 0; for (int k = 0; k < 3; k++) S[3 + k] = w->daxis[da][k]; }
+    cross_motion(Sd, v, S);
+    real qd = w->qvel[da];
+    for (int c = 0; c < 6; c++) { v[c] += S[c] * qd; a[c] += Sd[c] * qd; }
+  }
+}
+// body force f = I a + v x* (I v) of link l
+DEV void mw_rne_force(const MwModel* __restrict__ m, const WarpScratch* w, int l, const real* v, const real* a, real* f) {
+  real mass = m->link_mass[l];
+  for (int i = 0; i < 6; i++) f[i] = 0;
+  if (mass > 0) {
+    real c[3], t[3], u[3], Iw[9];      // from mw_link_inertia (mw_mass_matrix ran on the same poses)
+    for (int i = 0; i < 3; i++) c[i] = w->lcom[l][i];
+    for (int i = 0; i < 9; i++) Iw[i] = w->lIw[l][i];
+    real pl[3], Lm[3], pa[3], La[3];
+    v3cross(t, v, c); for (int i = 0; i < 3; i++) pl[i] = mass * (v[3 + i] + t[i]);
+    mat_mulvec(Lm, Iw, v); v3cross(t, c, pl); v3add(Lm, Lm, t);
+    v3cross(t, a, c); for (int i = 0; i < 3; i++) pa[i] = mass * (a[3 + i] + t[i]);
+    mat_mulvec(La, Iw, a); v3cross(t, c, pa); v3add(La, La, t);
+    v3cross(t, v, Lm); v3cross(u, v + 3, pl);
+    for (int i = 0; i < 3; i++) f[i] = La[i] + t[i] + u[i];
+    v3cross(t, v, pl);
+    for (int i = 0; i < 3; i++) f[3 + i] = pa[i] + t[i];
+  }
+}
 // returns qfrc_bias for this lane's dof.  Uses w->H as scratch (cvel/cacc/cfrc per link).
+// One link per lane: only the velocity / acceleration recursion depends on the parent, and it advances by tree depth (the
+// lanes of one level together); the body force of a link needs nothing but its own v and a, so all links compute theirs
+// at once.  -DMW_SERIAL_LINKS (see mw_kinematics) builds the form this replaces: every lane computes every link in index
+// order, lane 0 stores.  Same expressions in the same order either way: same bits.
 __device__ __noinline__ real mw_rne_bias(const MwModel* __restrict__ m, WarpScratch* w, const LaneDof& L, int lane) {
   real* cvel = w->H; real* cacc = w->H + 6 * MW_MAXLINK; real* cfrc = w->H + 12 * MW_MAXLINK;
   const int nl = m->nlink;
+#ifndef MW_SERIAL_LINKS
+  const int depth = lane < nl ? m->link_depth[lane] : -1, nd = m->ndepth;
+  real v[6], a[6], f[6];
+  for (int d = 0; d < nd; d++) {
+    if (depth == d) {
+      const int l = lane, p = m->link_parent[l];
+      if (p < 0) { for (int c = 0; c < 6; c++) { v[c] = 0; a[c] = 0; } a[3] = -m->gravity[0]; a[4] = -m->gravity[1]; a[5] = -m->gravity[2]; }
+      else { for (int c = 0; c < 6; c++) { v[c] = cvel[6 * p + c]; a[c] = cacc[6 * p + c]; } }
+      mw_rne_joint(m, w, l, v, a);
+      for (int c = 0; c < 6; c++) { cvel[6 * l + c] = v[c]; cacc[6 * l + c] = a[c]; }
+    }
+    SYNCW();
+  }
+  if (lane < nl) {
+    mw_rne_force(m, w, lane, v, a, f);
+    for (int c = 0; c < 6; c++) cfrc[6 * lane + c] = f[c];
+  }
+  SYNCW();
+#else
   for (int l = 0; l < nl; l++) {
     int p = m->link_parent[l];
-    real v[6], a[6];
+    real v[6], a[6], f[6];
     if (p < 0) { for (int c = 0; c < 6; c++) { v[c] = 0; a[c] = 0; } a[3] = -m->gravity[0]; a[4] = -m->gravity[1]; a[5] = -m->gravity[2]; }
     else { for (int c = 0; c < 6; c++) { v[c] = cvel[6 * p + c]; a[c] = cacc[6 * p + c]; } }
-    int jt = m->link_jtype[l], da = m->link_dadr[l];
-    if (jt == JT_FREE) {
-      real vb[6];
-      for (int i = 0; i < 3; i++) {   // world-fixed translation axes
-        real S[6] = {0, 0, 0, w->daxis[da + i][0], w->daxis[da + i][1], w->daxis[da + i][2]}, Sd[6];
-        cross_motion(Sd, v, S);
-        real qd = w->qvel[da + i];
-        for (int c = 0; c < 6; c++) { a[c] += Sd[c] * qd; }
-        for (int c = 0; c < 6; c++) v[c] += S[c] * qd;
-      }
-      for (int c = 0; c < 6; c++) vb[c] = v[c];
-      for (int i = 3; i < 6; i++) {   // body-fixed rotation axes: all three see the same velocity
-        real S[6], Sd[6];
-        for (int k = 0; k < 3; k++) S[k] = w->daxis[da + i][k];
-        v3cross(S + 3, w->danchor[da + i], w->daxis[da + i]);
-        cross_motion(Sd, vb, S);
-        real qd = w->qvel[da + i];
-        for (int c = 0; c < 6; c++) { a[c] += Sd[c] * qd; v[c] += S[c] * qd; }
-      }
-    } else {
-      real S[6], Sd[6];
-      if (jt == JT_HINGE) { for (int k = 0; k < 3; k++) S[k] = w->daxis[da][k]; v3cross(S + 3, w->danchor[da], w->daxis[da]); }
-      else { S[0] = S[1] = S[2] = 0; for (int k = 0; k < 3; k++) S[3 + k] = w->daxis[da][k]; }
-      cross_motion(Sd, v, S);
-      real qd = w->qvel[da];
-      for (int c = 0; c < 6; c++) { v[c] += S[c] * qd; a[c] += Sd[c] * qd; }
-    }
-    // body force f = I a + v x* (I v)
-    real mass = m->link_mass[l];
-    real f[6] = {0, 0, 0, 0, 0, 0};
-    if (mass > 0) {
-      real c[3], t[3], u[3], Iw[9];      // from mw_link_inertia (mw_mass_matrix ran on the same poses)
-      for (int i = 0; i < 3; i++) c[i] = w->lcom[l][i];
-      for (int i = 0; i < 9; i++) Iw[i] = w->lIw[l][i];
-      real pl[3], Lm[3], pa[3], La[3];
-      v3cross(t, v, c); for (int i = 0; i < 3; i++) pl[i] = mass * (v[3 + i] + t[i]);
-      mat_mulvec(Lm, Iw, v); v3cross(t, c, pl); v3add(Lm, Lm, t);
-      v3cross(t, a, c); for (int i = 0; i < 3; i++) pa[i] = mass * (a[3 + i] + t[i]);
-      mat_mulvec(La, Iw, a); v3cross(t, c, pa); v3add(La, La, t);
-      v3cross(t, v, Lm); v3cross(u, v + 3, pl);
-      for (int i = 0; i < 3; i++) f[i] = La[i] + t[i] + u[i];
-      v3cross(t, v, pl);
-      for (int i = 0; i < 3; i++) f[3 + i] = pa[i] + t[i];
-    }
+    mw_rne_joint(m, w, l, v, a);
+    mw_rne_force(m, w, l, v, a, f);
     if (lane == 0) for (int c = 0; c < 6; c++) { cvel[6 * l + c] = v[c]; cacc[6 * l + c] = a[c]; cfrc[6 * l + c] = f[c]; }
     SYNCW();
   }
+#endif
   // leaves-to-root accumulation of the link forces: the six components are independent, one lane each
   if (lane < 6) for (int l = nl - 1; l >= 0; l--) { int p = m->link_parent[l]; if (p >= 0) cfrc[6 * p + lane] += cfrc[6 * l + lane]; }
   SYNCW();
@@ -487,7 +613,11 @@ __device__ __noinline__ void mw_collide(const MwModel* __restrict__ m, const flo
       for (int i = 0; i < 9; i++) Rw[i] = Rl[i];
     } else {
       creal Lm[9], Lp[3], t[3];
+#ifndef MW_SERIAL_LINKS
+      for (int i = 0; i < 9; i++) Lm[i] = mw_lmatd(w, l)[i];     // quat2mat of lquatd[l], from mw_kinematics
+#else
       quat2mat(Lm, w->lquatd[l]);
+#endif
       for (int i = 0; i < 3; i++) Lp[i] = w->lposd[l][i];
       mat_mulvec(t, Lm, gp); v3add(pos, Lp, t);
       mat_mul(Rw, Lm, Rl);
@@ -1078,6 +1208,7 @@ __device__ __noinline__ void mw_forward(const MwModel* __restrict__ m, const flo
   // own work goes to prof[i]; the time spent waiting for the CTA's other warps at the phase boundary goes to prof[12]
 #define PROF_(i, b) { t1 = MW_CLK(w); if (lane == 0) w->prof[i] += t1 - t0; PHASE_SYNC_AT(b); t0 = MW_CLK(w); if (lane == 0) w->prof[12] += t0 - t1; }
   mw_kinematics(m, w, lane);
+  if (w->prof_on && lane == 0) w->prof[15] += mw_clock() - t0;
   LaneDof L; mw_lane_dof(m, w, lane, &L);
   mw_mass_matrix(m, w, L, lane);
   PROF_(0, 1)
@@ -1120,7 +1251,7 @@ __device__ __noinline__ void mw_forward_kinematics_only(const MwModel* __restric
   PHASE_SYNC_AT(0);
   t1 = MW_CLK(w); if (lane == 0) w->prof[12] += t1 - t0; t0 = t1;
   mw_kinematics(m, w, lane);
-  t1 = MW_CLK(w); if (lane == 0) w->prof[0] += t1 - t0;
+  t1 = MW_CLK(w); if (lane == 0) { w->prof[0] += t1 - t0; w->prof[15] += t1 - t0; }
   if (lane == 0) { w->solver_iter = 0; w->ncon_dropped = 0; }
   SYNCW();
 }

@@ -377,7 +377,7 @@ class Engine:
         return a[:, :ncw].reshape(self.n_envs, -1, 12), a[:, ncw:ncw + 17], a[:, ncw + 17:]
 
     PROFILE_KEYS = ["kin_mass", "collide", "gjk_epa", "constraints", "bias_smooth", "solver", "euler_glue", "obs_reward", "step",
-                    "n_convex_pairs", "n_epa_expansions", "n_gjk_iters", "barrier_wait", "n_sep_tested", "n_sep_rejected"]
+                    "n_convex_pairs", "n_epa_expansions", "n_gjk_iters", "barrier_wait", "n_sep_tested", "n_sep_rejected", "kin"]
 
     def profile(self):
         """Per-phase warp-cycle counters summed over all env steps since the last call (mw_get_profile)."""

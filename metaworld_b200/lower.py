@@ -38,12 +38,14 @@ NO_CSLOT = 255       # pair_cslot of a pair that never goes to GJK/EPA
 FIELDS = [
     ("qpos0d", "f8", (MAXNQ,)),     # float64 copy of qpos0 (mj_resetData must reproduce free-joint initial poses exactly)
     ("nlink", "i4", ()), ("nq", "i4", ()), ("nv", "i4", ()), ("ngeom", "i4", ()), ("npair", "i4", ()),
-    ("nframe", "i4", ()), ("nmeshvert", "i4", ()), ("pad0", "i4", ()),
+    ("nframe", "i4", ()), ("nmeshvert", "i4", ()),
+    ("ndepth", "i4", ()),           # levels of the link forest: 1 + the largest link_depth
     ("timestep", "f4", ()), ("solver_scale", "f4", ()), ("gravity", "f4", (3,)), ("tolerance", "f4", ()),
     ("impratio", "f4", ()), ("pad1", "f4", ()),
     # links
     ("link_parent", "i4", (MAXLINK,)), ("link_jtype", "i4", (MAXLINK,)), ("link_qadr", "i4", (MAXLINK,)),
     ("link_dadr", "i4", (MAXLINK,)), ("link_shift", "i4", (MAXLINK,)), ("link_dofmask", "u4", (MAXLINK,)),
+    ("link_depth", "i4", (MAXLINK,)),       # 0 for a root link, parent's + 1 otherwise (parents precede their children)
     ("link_pos", "f4", (MAXLINK, 3)), ("link_quat", "f4", (MAXLINK, 4)), ("link_jaxis", "f4", (MAXLINK, 3)),
     ("link_jpos", "f4", (MAXLINK, 3)), ("link_mass", "f4", (MAXLINK,)), ("link_com", "f4", (MAXLINK, 3)),
     ("link_inertia", "f4", (MAXLINK, 6)),
@@ -252,6 +254,8 @@ def lower(m: mjcf.Model, movable: str | None, task_frames=()) -> Lowered:
             d = cp - com
             It += Iw + mass * (np.dot(d, d) * np.eye(3) - np.outer(d, d))
         r["link_parent"][l] = L["parent"]
+        assert L["parent"] < l
+        r["link_depth"][l] = 0 if L["parent"] < 0 else r["link_depth"][L["parent"]] + 1
         r["link_jtype"][l] = L["jtype"]
         r["link_qadr"][l] = L["qadr"]
         r["link_dadr"][l] = L["dadr"]
@@ -294,6 +298,7 @@ def lower(m: mjcf.Model, movable: str | None, task_frames=()) -> Lowered:
     r["qpos0"][: m.nq] = a["qpos0"]
     r["qpos0d"][: m.nq] = a["qpos0"]
     r["nlink"], r["nq"], r["nv"] = nl, m.nq, nv
+    r["ndepth"] = int(r["link_depth"][:nl].max()) + 1
     r["timestep"] = m.opt["timestep"]
     r["solver_scale"] = 1.0 / (m.opt["meaninertia"] * max(1, nv))
     r["gravity"] = m.opt["gravity"]
