@@ -19,6 +19,9 @@ NVCC_TARGET = ["-gencode", "arch=compute_90a,code=sm_90a"]
 # operation exactly as written (DESIGN.md section 4, "Storage-independent results").
 NVCC_TARGET += ["--fmad=false"]
 HEADERS = ["mw_math.cuh", "mw_collide.cuh", "mw_physics.cuh", "mw_tasks.cuh", "mw_tasks_gen.cuh", "mw_policies.cuh"]
+# what every library is rebuilt from: the sources, the generated headers and the generators behind them, the C ABI header
+DEPS = [os.path.join(CSRC, f) for f in SOURCES + HEADERS + ["mw_model.h", "mw_task_ids.h"]] + [
+    os.path.join(_HERE, "lower.py"), os.path.join(_HERE, "tasks.py"), os.path.join(_HERE, "..", "include", "metaworld_b200.h")]
 
 
 def write_header():
@@ -38,54 +41,39 @@ def write_header():
     return path
 
 
-def needs_build():
-    if not os.path.exists(SO):
+def needs_build(path=SO):
+    """True when the library at `path` is missing or older than one of DEPS."""
+    if not os.path.exists(path):
         return True
-    t = os.path.getmtime(SO)
-    deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS + ["mw_model.h", "mw_task_ids.h"]] + [os.path.join(_HERE, "lower.py"), os.path.join(_HERE, "tasks.py"),
-            os.path.join(_HERE, "..", "include", "metaworld_b200.h")]
-    return any(os.path.exists(d) and os.path.getmtime(d) > t for d in deps)
+    t = os.path.getmtime(path)
+    return any(os.path.getmtime(d) > t for d in DEPS)
 
 
-def build(force=False, verbose=False, real_double=False, extra=()):
+def _nvcc(path, defines, verbose):
+    """Compiles the engine with -D`defines` into `path`."""
+    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+    cmd = [nvcc] + (["-Xptxas", "-v"] if verbose else []) + [f"-D{d}" for d in defines] + NVCC_TARGET + [
+        "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", path] + [os.path.join(CSRC, s) for s in SOURCES]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        sys.stderr.write(r.stdout + r.stderr)
+        raise RuntimeError(f"nvcc failed ({os.path.basename(path)})")
+    if verbose:
+        print(r.stdout + r.stderr)
+    return path
+
+
+def _build(path, defines, force, verbose):
     write_header()
-    if real_double:
-        return _build_f64(force, verbose)
-    if not force and not needs_build():
-        return SO
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc] + NVCC_TARGET + ["-O3", "-lineinfo", "-std=c++17", "--use_fast_math" if False else "-DMW_NO_FASTMATH",
-           "-Xcompiler", "-fPIC", "-shared", "-o", SO] + [os.path.join(CSRC, s) for s in SOURCES]
-    if real_double:
-        cmd.insert(1, "-DMW_REAL_DOUBLE")
-    if verbose:
-        cmd[1:1] = ["-Xptxas", "-v"]
-    cmd[1:1] = list(extra)
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(r.stdout + r.stderr)
-        raise RuntimeError("nvcc failed")
-    if verbose:
-        print(r.stdout + r.stderr)
-    return SO
+    if force or needs_build(path):
+        _nvcc(path, defines, verbose)
+    return path
 
 
-def _build_f64(force=False, verbose=False):
-    deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS + ["mw_model.h", "mw_task_ids.h"]] + [os.path.join(_HERE, "..", "include", "metaworld_b200.h")]
-    if not force and os.path.exists(SO_F64) and os.path.getmtime(SO_F64) >= max(os.path.getmtime(d) for d in deps if os.path.exists(d)):
-        return SO_F64
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc, "-DMW_REAL_DOUBLE", "-DWARPS_PER_BLOCK=3"] + NVCC_TARGET + ["-O3", "-lineinfo", "-std=c++17",
-           "-Xcompiler", "-fPIC", "-shared", "-o", SO_F64] + [os.path.join(CSRC, s) for s in SOURCES]
-    if verbose:
-        cmd[1:1] = ["-Xptxas", "-v"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(r.stdout + r.stderr)
-        raise RuntimeError("nvcc failed (f64 build)")
-    if verbose:
-        print(r.stdout + r.stderr)
-    return SO_F64
+def build(force=False, verbose=False, real_double=False):
+    if real_double:
+        return _build(SO_F64, ["MW_REAL_DOUBLE", "WARPS_PER_BLOCK=3"], force, verbose)
+    return _build(SO, [], force, verbose)
 
 
 def build_variant(path, defines=(), force=False):
@@ -93,7 +81,6 @@ def build_variant(path, defines=(), force=False):
     overflow path, whose results must be bit-identical to the standard build; tests/test_gpu.py).  Returns the library's
     path: `path`, or a file of the same name in a per-user temporary directory when `path`'s directory cannot be written
     (tests may run from a read-only checkout)."""
-    write_header()
     try:
         os.makedirs(os.path.dirname(path), exist_ok=True)
         writable = os.access(os.path.dirname(path), os.W_OK)
@@ -102,24 +89,15 @@ def build_variant(path, defines=(), force=False):
     if not writable:
         path = os.path.join(tempfile.gettempdir(), f"metaworld_b200-{os.getuid()}", os.path.basename(path))
         os.makedirs(os.path.dirname(path), exist_ok=True)
-    srcs = [os.path.join(CSRC, f) for f in SOURCES + HEADERS + ["mw_model.h", "mw_task_ids.h"]]
-    if not force and os.path.exists(path) and os.path.getmtime(path) >= max(os.path.getmtime(d) for d in srcs):
-        return path
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc] + [f"-D{d}" for d in defines] + NVCC_TARGET + ["-O3", "-lineinfo", "-std=c++17", "-DMW_NO_FASTMATH",
-                                                  "-Xcompiler", "-fPIC", "-shared", "-o", path] + [os.path.join(CSRC, s) for s in SOURCES]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(r.stdout + r.stderr)
-        raise RuntimeError("nvcc failed (variant build)")
-    return path
+    return _build(path, list(defines), force, False)
 
 
 if __name__ == "__main__":
+    verbose = "-v" in sys.argv
     if "--double" in sys.argv:
-        print(build(force=True, verbose="-v" in sys.argv, real_double=True))
+        print(build(force=True, verbose=verbose, real_double=True))
     elif "--single" in sys.argv:
-        print(build(force=True, verbose="-v" in sys.argv))
+        print(build(force=True, verbose=verbose))
     else:   # both libraries: the float32 step engine and the float64 snapshot builder
-        print(build(force=True, verbose="-v" in sys.argv))
-        print(_build_f64(True, "-v" in sys.argv))
+        print(build(force=True, verbose=verbose))
+        print(build(force=True, verbose=verbose, real_double=True))

@@ -896,10 +896,15 @@ int mw_sizeof_taskconst(void) { return (int)sizeof(MwTaskConst); }
 int mw_sizeof_envstate(void) { return (int)sizeof(MwEnvState); }
 int mw_sizeof_snapshot(void) { return (int)sizeof(MwSnapshot); }
 const char* mw_last_error(void) { return g_err.c_str(); }
+#ifdef MW_CHOL_ONE_CHAIN
+#define MW_CHOL_INFO " one-chain cholesky"
+#else
+#define MW_CHOL_INFO ""
+#endif
 const char* mw_build_info(void) {
   static char buf[256];
   snprintf(buf, sizeof(buf), "real=%s maxcon=%d(shared %d) maxefc=%d(shared %d) warps_per_block=%d smem_per_block=%zu%s", sizeof(real) == 4 ? "float" : "double",
-           MW_MAXCON, MW_SMCON, MW_MAXEFC, MW_SMEFC, WARPS_PER_BLOCK, smem_bytes(), MW_LINKS_INFO);
+           MW_MAXCON, MW_SMCON, MW_MAXEFC, MW_SMEFC, WARPS_PER_BLOCK, smem_bytes(), MW_LINKS_INFO MW_CHOL_INFO);
   return buf;
 }
 

@@ -201,8 +201,8 @@ __device__ __noinline__ void mw_kinematics(const MwModel* __restrict__ m, WarpSc
 }
 #else
 #define MW_LINKS_INFO " serial links"
-// The link-by-link form (-DMW_SERIAL_LINKS: the A arm of scripts/gpu_kin_ab.py and the reference of the bitwise tests, not
-// a supported configuration).  Sequential over the links; every lane computes the same values, lane 0 stores.
+// The link-by-link form (-DMW_SERIAL_LINKS: the A arm of `scripts/gpu_variant_ab.py -D MW_SERIAL_LINKS` and the reference
+// of the bitwise tests, not a supported configuration).  Sequential over the links; every lane computes the same values, lane 0 stores.
 __device__ __noinline__ void mw_kinematics(const MwModel* __restrict__ m, WarpScratch* w, int lane) {
   const int nl = m->nlink;
   double quat[4], R[9];          // orientation of the link in work; at the top of an iteration: of the previous link

@@ -1,8 +1,9 @@
 """Where the numpy-API step spends host time around the kernel (MT50 @ 4096, steady state)."""
-import sys, time, numpy as np, torch
-sys.path.insert(0, '.')
+import time, numpy as np, torch
 from types import SimpleNamespace
+from gpu_timing_common import card
 from bench import build_env, stagger
+print("card:", card())
 env, names, _, _ = build_env(SimpleNamespace(benchmark="MT50", envs_per_gpu=4096, seed=42), 0, 0)
 N = env.num_envs
 env.reset(); stagger(env, 0)

@@ -6,13 +6,12 @@ one `step_torch` of the same envs.  Times come from CUDA events around `reps` ba
 Prints one JSON line with the card name, its power limit and max SM clock, and writes it to <out>/query_timing.json
 when an output directory is given.  Usage (on a GPU):
     python scripts/gpu_query_timing.py [reps] [out_dir]"""
-import json, os, subprocess, sys
+import json, os, sys
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from metaworld_b200.vector_env import make_mt_envs  # noqa: E402
+from gpu_timing_common import card, steady_env, timed
 
 REPS = int(sys.argv[1]) if len(sys.argv) > 1 else 100
 OUT = sys.argv[2] if len(sys.argv) > 2 else None
@@ -22,33 +21,8 @@ SITES = ("rightEndEffector", "leftEndEffector", "goal", "hole", "handle")
 GEOMS = ("objGeom", "leftpad_geom", "rightpad_geom", "handle", "mug")       # 16 frames in all
 
 
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return {"torch_name": torch.cuda.get_device_name(0), "nvidia_smi": q[0] if q else None}
-
-
-def timed(fn, reps, warm=5):
-    for _ in range(warm):
-        fn()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    a.record()
-    for _ in range(reps):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / reps
-
-
 def main():
-    env = make_mt_envs("MT50", seed=42, num_envs=N, use_one_hot=True)
-    env.reset()
-    p = (np.arange(N) * 500 // N)[np.random.default_rng(0).permutation(N)]          # bench.stagger
-    st = env.engine.get_state()
-    st["path_len"] = p.astype(np.float32)
-    env.engine.set_state(st)
-    env._ep_len[:] = p
+    env = steady_env("MT50", N, use_one_hot=True)
     A = torch.from_numpy(np.random.default_rng(1).uniform(-1, 1, size=(N, 4)).astype(np.float32)).to(env.device)
     for _ in range(20):
         env.step_torch(A)

@@ -2,10 +2,15 @@
 A[nb:, :nb] is exactly zero, factoring / back-substituting the two diagonal blocks independently gives, element for element
 and bit for bit, what the single right-looking chain gives - the skipped work is exclusively `x -= l * 0`.  The model uses
 the kernel's operation order in float32 (numpy has no fused multiply-add: the statement is about dense vs block order within
-one arithmetic, which is what the device relies on; the device-side equality is checked on the GPU by per-step digests of
-the two builds, scripts/gpu_ab.py with -DMW_CHOL_ONE_CHAIN)."""
+one arithmetic, which is what the device relies on).  On the GPU, the default build and one built with -DMW_CHOL_ONE_CHAIN
+(never split the factorisation) give equal per-step digests of an MT50 rollout and an equal final state (scripts/gpu_ab.py).
+"Equal" is up to the sign of zero: the single chain's `x - l * 0`, which the two chains skip, can change the sign of a zero
+x, so some warm-start entries of the final state are -0.0 in one build and +0.0 in the other; no later operation can tell
+them apart."""
 import numpy as np
 import pytest
+
+from builds import run_digests, variant_lib
 
 f32 = np.float32
 
@@ -76,3 +81,16 @@ def test_coupled_blocks_need_the_single_chain():
     assert not np.allclose(np.tril(one)[nb:, nb:], np.tril(two)[nb:, nb:], atol=1e-3)
     coupled = bool(np.any(A[nb:, :nb] != 0))     # the run-time test of mw_chol
     assert coupled
+
+
+@pytest.mark.gpu
+def test_one_chain_cholesky_build_is_bitwise_identical(tmp_path):
+    """MT50 @ 4096 envs, 150 random-action steps: the default build (two chains where the coupling block is zero) against
+    -DMW_CHOL_ONE_CHAIN."""
+    import torch
+    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
+    a = run_digests(tmp_path / "two.json")
+    b = run_digests(tmp_path / "one.json", variant_lib("MW_CHOL_ONE_CHAIN"))
+    assert "one-chain cholesky" in b["build"] and "one-chain cholesky" not in a["build"]
+    assert a["steps"] == b["steps"] and a["state_values"] == b["state_values"]
+    assert a["dropped"] == b["dropped"] == 0

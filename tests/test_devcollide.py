@@ -5,10 +5,11 @@ so the exact statements that run on the GPU (analytic pairs, aligned cylinder fa
 its index-ordered compaction) are exercised here, without a GPU, on identical float64 inputs."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
+
+from builds import host_shim
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -18,13 +19,10 @@ G_PLANE, G_SPHERE, G_CAPSULE, G_CYLINDER, G_BOX, G_MESH = 0, 2, 3, 5, 6, 7
 
 @pytest.fixture(scope="module")
 def libs():
-    src = os.path.join(HERE, "devcollide", "shim.cpp")
-    deps = [src] + [os.path.join(ROOT, "metaworld_b200", "csrc", f) for f in ("mw_collide.cuh", "mw_math.cuh")]
-    if not os.path.exists(SHIM) or os.path.getmtime(SHIM) < max(os.path.getmtime(d) for d in deps):
-        subprocess.run(["g++", "-O2", "-fPIC", "-shared", "-std=c++17", "-w", "-o", SHIM, src], check=True)
+    shim = host_shim("devcollide", SHIM, headers=("mw_collide.cuh", "mw_math.cuh"))
     from oracle import mjphys
     mjphys.build()
-    return C.CDLL(SHIM), C.CDLL(os.path.join(ROOT, "oracle", "libmjphys.so"))
+    return shim, C.CDLL(os.path.join(ROOT, "oracle", "libmjphys.so"))
 
 
 def _call(fn, dev, t1, p1, m1, s1, v1, t2, p2, m2, s2, v2, margin):

@@ -5,54 +5,16 @@ physics, tests/golden/make_reference_goldens.py), (b) the live CPU oracle on fre
 
 Tolerances (float32 device vs float64 oracle): 1e-4 absolute on observations and rewards, as BASELINE.json's
 north_star states; success flags must be equal.  PARITY UNPINNED w.r.t. MuJoCo itself (see oracle/mjphys.h)."""
-import glob
 import os
 
 import numpy as np
 import pytest
 
+from builds import run_digests, variant_lib
+from rig import (GOLD, POLICY_FAILS_ON_REFERENCE_GLUE, SENSITIVE_CONTACT_RICH, SENSITIVE_ONE_STEP, SENSITIVE_OPEN_LOOP,
+                 SENSITIVE_RESET, TOL, Rig, _TOUCH, _params, _report, _tasks_with_goldens)
+
 pytestmark = pytest.mark.gpu
-GOLD = os.path.join(os.path.dirname(__file__), "golden")
-TOL = 1e-4
-
-
-def _tasks_with_goldens():
-    from metaworld_b200.tasks import TASKS
-    names = [os.path.basename(p)[5:-4] for p in sorted(glob.glob(os.path.join(GOLD, "traj_*.npz")))]
-    return [n for n in names if n in TASKS]
-
-
-# Known float32-vs-float64 sensitivities (measured, see DESIGN.md section 7).  These are
-# reported as xfail with the reason, never skipped: each one is a place where contact dynamics amplify a 1e-7 state
-# difference (an object jammed in a hole, a nut resting on a peg, an object that starts exactly touching a surface so
-# that `dist < margin` is decided by the last bit), not a missing feature.
-_JAMMED = "resting contacts under load are chaotic: float32 step vs float64 oracle diverge beyond 1e-4 within the rollout"
-_TOUCH = "object starts exactly touching (dist == margin to the last bit): contact inclusion differs between float32 and float64 state"
-SENSITIVE_RESET = {"disassemble-v3": _JAMMED, "peg-unplug-side-v3": _JAMMED}
-SENSITIVE_OPEN_LOOP = {"assembly-v3": _JAMMED, "basketball-v3": _TOUCH, "box-close-v3": _JAMMED, "coffee-push-v3": _JAMMED,
-                       "disassemble-v3": _JAMMED,
-                       "peg-unplug-side-v3": "the plug starts jammed in its socket (SENSITIVE_RESET): the rollout amplifies any change of float32 rounding "
-                                             "(e.g. a different FMA contraction after a refactor) to ~3e-4 within 60 steps; single steps agree to 3e-5 (contact-rich test)",
-                       "handle-press-v3": "observations agree to 3e-6; the reward (slope ~50 near the handle) turns that into 1.4e-4",
-                       "drawer-close-v3": "goal 0's golden trajectory passes 1.07e-7 m from a contact-activation discontinuity (the left claw grazes the drawer front inside the "
-                                          "1 mm margin at step 2): the float64 oracle itself jumps by 1.08e-4 when the drawer is moved by 1.08e-7 "
-                                          "(tests/test_oracle.py::test_drawer_close_golden_knife_edge); float32 state noise puts the device on the other side"}
-SENSITIVE_ONE_STEP = {"assembly-v3": "the nut rests on the peg (mesh-cylinder contacts under load): single steps reach 1.2e-4"}
-SENSITIVE_CONTACT_RICH = {"soccer-v3": "mesh-mesh face contact (hand against the goal frame): EPA witness point on a flat patch is path dependent"}
-
-
-def _report(name, row):
-    """Appends one measurement row to $MW_TEST_REPORT_DIR/<name> when that variable names a directory to collect them in."""
-    d = os.environ.get("MW_TEST_REPORT_DIR")
-    if d:
-        os.makedirs(d, exist_ok=True)
-        with open(os.path.join(d, name), "a") as f:
-            f.write(row)
-
-
-def _params(sensitive):
-    return [pytest.param(t, marks=pytest.mark.xfail(reason=sensitive[t], strict=False)) if t in sensitive else t
-            for t in _tasks_with_goldens()]
 
 
 @pytest.fixture(scope="module")
@@ -60,34 +22,6 @@ def torch_cuda():
     import torch
     assert torch.cuda.is_available(), "GPU tests need a CUDA device"
     return torch
-
-
-class Rig:
-    """N envs of one task, driven through the raw engine (C ABI)."""
-
-    def __init__(self, torch, task, rand_vecs, partial=False):
-        from metaworld_b200.engine import Engine
-        self.t = torch
-        self.eng = Engine([task])
-        n = len(rand_vecs)
-        self.ids = self.eng.build_snapshots([0] * n, rand_vecs, [int(partial)] * n)
-        self.eng.set_envs([0] * n)
-        self.eng.set_options(500, False, 0)
-        d = self.eng.device
-        self.n = n
-        self.obs = torch.zeros(n, 39, device=d); self.rew = torch.zeros(n, device=d)
-        self.term = torch.zeros(n, dtype=torch.uint8, device=d); self.trunc = torch.zeros(n, dtype=torch.uint8, device=d)
-        self.info = torch.zeros(n, 7, device=d); self.fobs = torch.zeros(n, 39, device=d); self.finfo = torch.zeros(n, 8, device=d)
-        self.sid = torch.tensor(self.ids, dtype=torch.int32, device=d)
-
-    def reset(self):
-        self.eng.reset(self.sid, self.obs)
-        return self.obs.cpu().numpy()
-
-    def step(self, a):
-        self.eng.step(self.t.tensor(np.ascontiguousarray(a, dtype=np.float32), device=self.eng.device), self.obs, self.rew, self.term,
-                      self.trunc, self.info, self.fobs, self.finfo, self.sid)
-        return self.obs.cpu().numpy(), self.rew.cpu().numpy(), self.info.cpu().numpy(), self.term.cpu().numpy(), self.trunc.cpu().numpy()
 
 
 @pytest.mark.parametrize("task", _params(SENSITIVE_RESET))
@@ -128,15 +62,9 @@ def test_teacher_forced_one_step(torch_cuda, task):
     rig = Rig(torch_cuda, task, g["rand_vec"])
     rig.reset()
     rig.step(g["actions"][:, 0])        # first step from reset, like the golden: state latched on the first reward call (bin-picking) latches here
-    nq, nv = g["qpos"].shape[2], g["qvel"].shape[2]
     worst = 0.0
     for t in range(0, g["actions"].shape[1] - 1, 7):
-        st = rig.eng.get_state()
-        for k in range(rig.n):
-            st[k]["qpos"][:nq] = g["qpos"][k, t]; st[k]["qvel"][:nv] = g["qvel"][k, t]
-            st[k]["mocap_pos"] = g["mocap"][k, t]; st[k]["prev_obs"] = g["obs"][k, t][:18]
-            st[k]["warm"][:] = 0; st[k]["path_len"] = t + 1
-        rig.eng.set_state(st)
+        rig.load_golden(g, t)
         o, r, info, _, _ = rig.step(g["actions"][:, t + 1])
         worst = max(worst, np.abs(o - g["obs"][:, t + 1]).max(), np.abs(r - g["reward"][:, t + 1]).max(),
                     np.abs(info - g["info"][:, t + 1]).max())
@@ -160,16 +88,10 @@ def test_teacher_forced_contact_rich(torch_cuda, task):
     rig = Rig(torch_cuda, task, g["p_rand_vec"])
     rig.reset()
     rig.step(g["p_actions"][:, 0])      # first step from reset, like the oracle: rewards with state latched on their first call (bin-picking) latch here
-    nq, nv = g["p_qpos"].shape[2], g["p_qvel"].shape[2]
     errs = []
     T = g["p_actions"].shape[1]
     for t in range(0, T - 1):
-        st = rig.eng.get_state()
-        for k in range(rig.n):
-            st[k]["qpos"][:nq] = g["p_qpos"][k, t]; st[k]["qvel"][:nv] = g["p_qvel"][k, t]
-            st[k]["mocap_pos"] = g["p_mocap"][k, t]; st[k]["prev_obs"] = g["p_obs"][k, t][:18]
-            st[k]["warm"][:] = 0; st[k]["path_len"] = t + 1
-        rig.eng.set_state(st)
+        rig.load_golden(g, t, "p_")
         o, r, info, _, _ = rig.step(g["p_actions"][:, t + 1])
         errs.append(np.maximum.reduce([np.abs(o - g["p_obs"][:, t + 1]).max(axis=1), np.abs(r - g["p_reward"][:, t + 1]),
                                        np.abs(info - g["p_info"][:, t + 1]).max(axis=1)]))       # obs, reward, all 7 info keys
@@ -540,10 +462,6 @@ def test_heterogeneous_mt50_batch_is_bitwise_the_per_task_result(torch_cuda):
 # the reference's acceptance test (tests/metaworld/envs/mujoco/sawyer_xyz/test_scripted_policies.py:10-35) needs the
 # reference's policy code, which is not on the GPU box and may not be copied.  Its closed-loop ACTIONS on the reference
 # glue (fixture keys `s_*`, 5 goals per task, run until success) are replayed open-loop on the device instead.
-POLICY_FAILS_ON_REFERENCE_GLUE = {"basketball-v3": "the reference's own policy scores 0/5 on the reference glue (DESIGN.md section 8: target aliasing)",
-                                  "peg-insert-side-v3": "the reference's own policy scores 3/5 on the reference glue with these goals"}
-
-
 @pytest.mark.parametrize("task", [pytest.param(t, marks=pytest.mark.xfail(reason=POLICY_FAILS_ON_REFERENCE_GLUE[t], strict=False))
                                   if t in POLICY_FAILS_ON_REFERENCE_GLUE else t for t in _tasks_with_goldens()])
 def test_scripted_policy_actions_succeed(torch_cuda, task):
@@ -717,22 +635,8 @@ def test_contact_overflow_path_is_bitwise_identical(torch_cuda, tmp_path):
     global memory and the pass runs the <SP = true> instantiation of the constraint code.  Built with a shared capacity of 6
     contacts (48 rows) nearly every env takes that path in nearly every pass; obs / reward / info digests of a 120-step MT10
     rollout and the final device state must equal the standard build's bit for bit."""
-    import json, subprocess, sys
-    from metaworld_b200 import build as B
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    var = B.build_variant(os.path.join(root, "tests", "_build", "libmwb200_smcon6.so"), ["MW_SMCON=6"])
-    outs = []
-    for name, lib in (("std", None), ("smcon6", var)):
-        env = dict(os.environ)
-        if lib:
-            env["MW_B200_LIB"] = lib
-        else:
-            env.pop("MW_B200_LIB", None)
-        out = str(tmp_path / f"{name}.json")
-        r = subprocess.run([sys.executable, os.path.join(root, "scripts", "gpu_ab.py"), out, "120", "MT10", "350"], cwd=root, env=env, capture_output=True, text=True, timeout=600)
-        assert r.returncode == 0, r.stdout + r.stderr
-        outs.append(json.load(open(out)))
-    a, b = outs
+    a = run_digests(tmp_path / "std.json", steps=120, benchmark="MT10", envs=350)
+    b = run_digests(tmp_path / "smcon6.json", variant_lib("MW_SMCON=6"), steps=120, benchmark="MT10", envs=350)
     assert "shared 48" in a["build"] and "shared 6" in b["build"]
     assert a["steps"] == b["steps"] and a["state"] == b["state"] and a["dropped"] == b["dropped"] == 0
 
@@ -742,19 +646,8 @@ def test_head_split_is_pure_scheduling(torch_cuda, tmp_path):
     by two CTAs of 4 + 3 warps while its predicted duration exceeds that fraction of the balanced SM load.  Which CTA an env
     runs in must not show in any output: per-step digests of obs / reward / info of an MT50 @ 4096 rollout (150 lock-step
     steps: late enough for the peg-unplug / box-close heads to be split) and the final device state equal the unsplit run's."""
-    import json, subprocess, sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    outs = []
-    for name, frac in (("off", None), ("split", "0.85")):
-        env = dict(os.environ)
-        env.pop("MW_B200_LIB", None); env.pop("MW_B200_SPLIT_FRAC", None)
-        if frac:
-            env["MW_B200_SPLIT_FRAC"] = frac
-        out = str(tmp_path / f"{name}.json")
-        r = subprocess.run([sys.executable, os.path.join(root, "scripts", "gpu_ab.py"), out], cwd=root, env=env, capture_output=True, text=True, timeout=600)
-        assert r.returncode == 0, r.stdout + r.stderr
-        outs.append(json.load(open(out)))
-    a, b = outs
+    a = run_digests(tmp_path / "off.json")
+    b = run_digests(tmp_path / "split.json", switches={"MW_B200_SPLIT_FRAC": "0.85"})
     assert a["steps"] == b["steps"] and a["state"] == b["state"] and a["dropped"] == b["dropped"] == 0
 
 

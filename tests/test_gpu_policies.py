@@ -11,7 +11,7 @@ import os
 import numpy as np
 import pytest
 
-from test_gpu import POLICY_FAILS_ON_REFERENCE_GLUE, _report
+from rig import POLICY_FAILS_ON_REFERENCE_GLUE, _report
 from test_policies import ALL_SOURCES, build_shim, expert_rows, host_actions
 
 pytestmark = pytest.mark.gpu

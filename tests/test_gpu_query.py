@@ -5,7 +5,7 @@ import os
 import numpy as np
 import pytest
 
-from test_gpu import GOLD, Rig, _tasks_with_goldens
+from rig import GOLD, Rig, _tasks_with_goldens
 from test_gpu_set_state import _steady_mt50
 
 pytestmark = pytest.mark.gpu

@@ -5,7 +5,7 @@ import os
 import numpy as np
 import pytest
 
-from test_gpu import GOLD, SENSITIVE_OPEN_LOOP, TOL, Rig, _params
+from rig import GOLD, SENSITIVE_OPEN_LOOP, TOL, Rig, _params
 
 pytestmark = pytest.mark.gpu
 

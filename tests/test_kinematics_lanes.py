@@ -8,17 +8,12 @@ CPU test: the CUDA source is compiled for the host with a 32-lane warp emulated 
 not CUDA's, but both forms call the same one; what is checked is that no operand, order or rounding differs.
 GPU test: per-step digests of an MT50 rollout and the final device state of the two builds (scripts/gpu_ab.py)."""
 import ctypes as C
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-CSRC = os.path.join(ROOT, "metaworld_b200", "csrc")
+from builds import host_shim, run_digests, variant_lib
+
 JT_FREE, JT_SLIDE, JT_HINGE = 0, 2, 3
 
 
@@ -55,11 +50,8 @@ def shims(tmp_path_factory):
     B.write_header()
     out = tmp_path_factory.mktemp("kinlanes")
     libs = []
-    for tag, defs in (("lanes", []), ("serial", ["-DMW_SERIAL_LINKS"])):
-        so = str(out / f"libkin_{tag}.so")
-        subprocess.run(["g++", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-std=c++17", "-w", *defs, "-o", so,
-                        os.path.join(HERE, "kinlanes", "shim.cpp")], check=True)
-        lib = C.CDLL(so)
+    for tag, defs in (("lanes", ()), ("serial", ("MW_SERIAL_LINKS",))):
+        lib = host_shim("kinlanes", str(out / f"libkin_{tag}.so"), defs)
         lib.kin_pass.restype = C.c_int
         libs.append(lib)
     return libs
@@ -110,20 +102,8 @@ def test_serial_links_build_is_bitwise_identical_on_mt50(tmp_path):
     """MT50 @ 4096 envs, 40 random-action steps: the default build against -DMW_SERIAL_LINKS."""
     import torch
     assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    from metaworld_b200 import build as B
-    serial = B.build_variant(os.path.join(ROOT, "tests", "_build", "libmwb200_seriallinks.so"), ["MW_SERIAL_LINKS"])
-    res = {}
-    for tag, lib in (("lanes", None), ("serial", serial)):
-        env = dict(os.environ)
-        env.pop("MW_B200_LIB", None); env.pop("MW_B200_SPLIT_FRAC", None)
-        if lib:
-            env["MW_B200_LIB"] = lib
-        out = str(tmp_path / f"{tag}.json")
-        r = subprocess.run([sys.executable, os.path.join(ROOT, "scripts", "gpu_ab.py"), out, "40"], cwd=ROOT, env=env,
-                           capture_output=True, text=True, timeout=900)
-        assert r.returncode == 0, r.stdout + r.stderr
-        res[tag] = json.load(open(out))
-    a, b = res["lanes"], res["serial"]
+    a = run_digests(tmp_path / "lanes.json", steps=40)
+    b = run_digests(tmp_path / "serial.json", variant_lib("MW_SERIAL_LINKS"), steps=40)
     assert "serial links" in b["build"] and "serial links" not in a["build"]
     assert a["steps"] == b["steps"] and a["state"] == b["state"]
     assert a["dropped"] == b["dropped"] == 0

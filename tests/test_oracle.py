@@ -389,7 +389,7 @@ def test_contact_jacobian_is_the_rate_of_change_of_distance():
 
 
 def test_drawer_close_golden_knife_edge():
-    """Evidence for the drawer-close entry of tests/test_gpu.py::SENSITIVE_OPEN_LOOP.  Goal 0 of the committed golden rollout
+    """Evidence for the drawer-close entry of tests/rig.py::SENSITIVE_OPEN_LOOP.  Goal 0 of the committed golden rollout
     sits on a contact discontinuity: at step 2 the left claw (a box) grazes the drawer front (a box with exactly parallel
     faces) inside the 1 mm margin while moving at ~1 m/s, and which box-box feature pair fires - hence whether the full
     damping impulse is applied once more - flips back and forth under sub-micrometre displacements of the drawer.  The

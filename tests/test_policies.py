@@ -10,29 +10,24 @@ to identical bits).  Two references:
 import ctypes as C
 import hashlib
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from builds import host_shim
+
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 GOLD = os.path.join(HERE, "golden")
-SRC = os.path.join(HERE, "devpolicy", "shim.cpp")
 # the observation rows of the expert-action fixture, in this order: resets and 60-step random-action rollouts, the
 # policy-driven rollouts (they reach the later branches of the decision trees), the partially observable rollout
 EXPERT_SOURCES = ("reset_obs", "obs", "p_reset_obs", "p_obs", "po_reset_obs", "po_obs")
 # every observation of a trajectory golden, the 500-step episode included (no reference actions needed: kernel vs host)
 ALL_SOURCES = EXPERT_SOURCES + ("l_reset_obs", "l_obs")
-DEPS = [SRC] + [os.path.join(ROOT, "metaworld_b200", "csrc", f) for f in ("mw_policies.cuh", "mw_task_ids.h")]
 
 
 def build_shim(path):
     """The host build of mw_policies.cuh at `path`, rebuilt when a source is newer."""
-    if not os.path.exists(path) or os.path.getmtime(path) < max(os.path.getmtime(d) for d in DEPS):
-        os.makedirs(os.path.dirname(path), exist_ok=True)
-        subprocess.run(["g++", "-O2", "-fPIC", "-shared", "-std=c++17", "-ffp-contract=off", "-o", path, SRC], check=True)
-    return C.CDLL(path)
+    return host_shim("devpolicy", path, headers=("mw_policies.cuh", "mw_task_ids.h"))
 
 
 def expert_rows(task, sources=EXPERT_SOURCES):
