@@ -115,6 +115,23 @@ int mw_set_physics(mw_engine*, const unsigned char* mask, const double* qpos, co
  * synchronisation: qpos DEV f64 [n_envs, 18], qvel DEV f64 [n_envs, 17] (the float32 record widened); columns past the
  * env's nq / nv are zero.                                                                                         */
 int mw_get_physics(mw_engine*, double* qpos, double* qvel, void* stream);
+/* Saved env states (no reference counterpart; the closest is SawyerMocapBase.__getstate__ / __setstate__,
+ * metaworld/sawyer_xyz_env.py:109-131, which keeps qpos / qvel only).  For every env i with mask[i] != 0 (mask NULL: all
+ * envs) mw_save_states copies the whole 512-byte state record (physics, warm start, mocap target, frame stack, reward
+ * latches, target, path length, episode counter and return, snapshot id, ended mark) into row i of `records`, the env's
+ * model slot into record_model[i] and its MW_NCONV separating-axis hints into row i of `hints`.  The hints never change a
+ * result (a stale one can only fail to reject a pair); they keep a loaded state's collision pass as cheap as its source's.
+ * mw_load_states gives every env i with mask[i] != 0 record src[i] (src NULL: record i) and its hints, so that the env
+ * continues bit for bit as the env it was saved from; an env whose src[i] is outside [0, n_records) or whose record holds
+ * another model slot is left unchanged and gets MW_FAULT_BAD_LOAD.  Fault bits, counters, profiles and the launch-order
+ * keys are not part of a saved state.  `records` must not overlap the engine's own state (forking from the live state
+ * is a save, then a load).  Neither call allocates or synchronises.  MW_ERR_ARG for a NULL engine or buffer and for
+ * n_records < 0.
+ *   mask DEV u8 [n_envs] or NULL; records DEV [n_records, 512 B]; record_model DEV i32 [n_records];
+ *   hints DEV f32 [n_records, MW_NCONV (128), 4]; src DEV i32 [n_envs] or NULL.                                       */
+int mw_save_states(mw_engine*, const unsigned char* mask, void* records, int* record_model, float* hints, void* stream);
+int mw_load_states(mw_engine*, const unsigned char* mask, const int* src, int n_records, const void* records,
+                   const int* record_model, const float* hints, void* stream);
 /* SawyerXYZEnv._get_obs() (metaworld/sawyer_xyz_env.py:513-527) of the current state for every env with mask[i] != 0:
  * kinematics, then the frame-stacked observation, unclipped as in the reference (step() clips afterwards); like the
  * reference it makes the current frame the env's prev_obs.  obs DEV float [n_envs, obs_stride]: row i (first 39
@@ -157,7 +174,9 @@ int mw_expert_actions(const int* task_ids, const float* obs, int obs_stride, int
  *   4 MW_FAULT_HAMACHER    hamacher_product input outside [0, 1]          (ValueError, reward_utils.py:237-238)
  *   8 MW_FAULT_NONFINITE   non-finite observation or reward (the reference's `_did_see_sim_exception` path)
  *  16 MW_FAULT_STEP_AFTER_END  DISABLED autoreset: stepped after its episode ended, before mw_reset_masked (gymnasium's
- *                              SyncVectorEnv asserts; SawyerXYZEnv.step raises past max_path_length).  API misuse.   */
+ *                              SyncVectorEnv asserts; SawyerXYZEnv.step raises past max_path_length).  API misuse.
+ *  32 MW_FAULT_BAD_LOAD    mw_load_states: the env's source record is out of range or holds another model slot; the env
+ *                          was left unchanged.  API misuse.                                                          */
 int mw_get_faults(mw_engine*, int* out);
 
 /* options: max_episode_steps (TimeLimit), terminate_on_success (0/1), device sampler seed */

@@ -495,6 +495,36 @@ __global__ void k_set_physics(EngineDev e, const int* __restrict__ env_model, co
   if (lane < m->nv) e.state[env].qvel[lane] = (float)qvel[(size_t)env * MW_MAXDOF + lane];
 }
 
+// Saved states (mw_save_states / mw_load_states), one warp per row: the 512-byte record moves as one float4 per lane, the
+// row's MW_NCONV separating-axis hints as MW_NCONV / 32 float4 per lane.  mask NULL = every row.
+__global__ void k_save_states(EngineDev e, const int* __restrict__ env_model, const unsigned char* __restrict__ mask,
+                              float4* __restrict__ records, int* __restrict__ record_model, float4* __restrict__ hints) {
+  const int env = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (env >= e.n_envs || (mask && !mask[env])) return;
+  records[(size_t)env * 32 + lane] = ((const float4*)(e.state + env))[lane];
+  for (int k = lane; k < MW_NCONV; k += 32) hints[(size_t)env * MW_NCONV + k] = e.sep_hint[(size_t)env * MW_NCONV + k];
+  if (lane == 0) record_model[env] = env_model[env];
+}
+
+// row env takes record src[env] (NULL: record env) and its hints when that record exists and holds a state of the row's
+// model; otherwise the row is left as it is and flagged MW_FAULT_BAD_LOAD.  `records` must not alias the engine's state.
+__global__ void k_load_states(EngineDev e, const int* __restrict__ env_model, const unsigned char* __restrict__ mask,
+                              const int* __restrict__ src, int n_records, const float4* __restrict__ records,
+                              const int* __restrict__ record_model, const float4* __restrict__ hints) {
+  const int env = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (env >= e.n_envs || (mask && !mask[env])) return;
+  int s = 0, ok = 0;
+  if (lane == 0) {
+    s = src ? src[env] : env;
+    ok = s >= 0 && s < n_records && record_model[s] == env_model[env];
+    if (!ok) e.diag[3 * env + 2] |= MW_FAULT_BAD_LOAD;
+  }
+  s = __shfl_sync(0xffffffffu, s, 0);
+  if (!__shfl_sync(0xffffffffu, ok, 0)) return;
+  ((float4*)(e.state + env))[lane] = records[(size_t)s * 32 + lane];
+  for (int k = lane; k < MW_NCONV; k += 32) e.sep_hint[(size_t)env * MW_NCONV + k] = hints[(size_t)s * MW_NCONV + k];
+}
+
 // SawyerMocapBase.get_env_state for every env: qpos [n_envs, MW_MAXNQ] float64, qvel [n_envs, MW_MAXDOF] widened to
 // float64; columns past the model's nq / nv are zero
 __global__ void k_get_physics(EngineDev e, const int* __restrict__ env_model, double* __restrict__ qpos, double* __restrict__ qvel) {
@@ -878,7 +908,7 @@ static int read_diag(const mw_engine* E, std::vector<int>& diag) {
   return 0;
 }
 
-// one warp per row (k_reset, k_reset_masked, k_set_physics, k_get_physics)
+// one warp per row (k_reset, k_reset_masked, k_set_physics, k_get_physics, k_save_states, k_load_states)
 #define ROW_THREADS 256
 static int row_blocks(int rows) { return (rows * 32 + ROW_THREADS - 1) / ROW_THREADS; }
 
@@ -1090,6 +1120,25 @@ int mw_get_physics(mw_engine* E, double* qpos, double* qvel, void* stream) {
   if (!qpos || !qvel) return fail(MW_ERR_ARG, "mw_get_physics: bad arguments");
   CK(cudaSetDevice(E->device));
   k_get_physics<<<row_blocks(E->n_envs), ROW_THREADS, 0, (cudaStream_t)stream>>>(E->dev(), E->d_env_model.p, qpos, qvel);
+  return launched(E, 1);
+}
+
+int mw_save_states(mw_engine* E, const unsigned char* mask, void* records, int* record_model, float* hints, void* stream) {
+  if (!E || !records || !record_model || !hints) return fail(MW_ERR_ARG, "mw_save_states: bad arguments");
+  if (!E->d_state.p) return fail(MW_ERR_STATE, "mw_save_states: mw_set_envs not called");
+  CK(cudaSetDevice(E->device));
+  k_save_states<<<row_blocks(E->n_envs), ROW_THREADS, 0, (cudaStream_t)stream>>>(E->dev(), E->d_env_model.p, mask, (float4*)records,
+                                                                                 record_model, (float4*)hints);
+  return launched(E, 1);
+}
+
+int mw_load_states(mw_engine* E, const unsigned char* mask, const int* src, int n_records, const void* records, const int* record_model,
+                   const float* hints, void* stream) {
+  if (!E || !records || !record_model || !hints || n_records < 0) return fail(MW_ERR_ARG, "mw_load_states: bad arguments");
+  if (!E->d_state.p) return fail(MW_ERR_STATE, "mw_load_states: mw_set_envs not called");
+  CK(cudaSetDevice(E->device));
+  k_load_states<<<row_blocks(E->n_envs), ROW_THREADS, 0, (cudaStream_t)stream>>>(E->dev(), E->d_env_model.p, mask, src, n_records,
+                                                                                 (const float4*)records, record_model, (const float4*)hints);
   return launched(E, 1);
 }
 

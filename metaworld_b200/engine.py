@@ -30,6 +30,7 @@ ENVSTATE_DTYPE = np.dtype([("qpos", "f8", 18), ("qvel", "f4", 17), ("warm", "f4"
                            ("ended", "f4"), ("gripper_ctrl", "f4"), ("pad", "f4", 2)])
 SNAPSHOT_DTYPE = np.dtype([("st", ENVSTATE_DTYPE), ("obs", "f4", 39), ("pad", "f4", 25)])
 MAXNQ, MAXDOF = 18, 17      # the padded qpos / qvel layout of set_physics / get_physics (ENVSTATE_DTYPE's qpos / qvel)
+NCONV = lower.MAXCONV       # separating-axis hints per env (MW_NCONV): a saved state's hint rows are [NCONV, 4] float32
 INFO_KEYS = ["success", "near_object", "grasp_success", "grasp_reward", "in_place_reward", "obj_to_target",
              "unscaled_reward"]
 
@@ -71,6 +72,8 @@ def _load(path):
     L.mw_set_physics.argtypes = [vp, vp, vp, vp, vp]
     L.mw_get_physics.argtypes = [vp, vp, vp, vp]
     L.mw_observe.argtypes = [vp, vp, vp, ip, vp]
+    L.mw_save_states.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.mw_load_states.argtypes = [vp, vp, vp, ip, vp, vp, vp, vp]
     L.mw_expert_actions.argtypes = [vp, vp, ip, ip, vp, vp]
     L.mw_query.argtypes = [vp, vp, vp, vp, ip, vp, vp, vp, vp]
     L.mw_get_faults.argtypes = [vp, vp]
@@ -299,6 +302,19 @@ class Engine:
         (float32 device tensor [n_envs, >= 39]); commits their frame stack (mw_observe)."""
         _ck(lib().mw_observe(self.h, self._p(mask), self._p(obs), obs.stride(0), self._stream()))
 
+    def save_states(self, records, record_model, hints, mask=None):
+        """Copies the state record, model slot and separating-axis hints of every env with `mask` set (bool device tensor
+        [n_envs]; None = all) into their rows of `records` (uint8 [n, 512]), `record_model` (int32 [n]) and `hints`
+        (float32 [n, NCONV, 4]), contiguous device tensors with n >= n_envs (mw_save_states)."""
+        _ck(lib().mw_save_states(self.h, self._p(mask), self._p(records), self._p(record_model), self._p(hints), self._stream()))
+
+    def load_states(self, records, record_model, hints, mask=None, src=None):
+        """Every env e with `mask` set (None = all) takes row `src[e]` (int32 device tensor [n_envs]; None = row e) of the
+        `save_states` buffers; a row out of range or of another model leaves the env unchanged and sets fault bit 32
+        (mw_load_states)."""
+        _ck(lib().mw_load_states(self.h, self._p(mask), self._p(src), records.shape[0], self._p(records), self._p(record_model),
+                                 self._p(hints), self._stream()))
+
     def query(self, mask, frame=None, pose=None, frames=None, touching=None, main_geom=None):
         """Read-only accessors of the current state for the envs with `mask` set (mw_query), into the given device tensors;
         each output may be None.  `frame` float32 [n_envs, 18]: columns 0..17 of the next `observe`, without committing
@@ -332,7 +348,8 @@ class Engine:
               4: "hamacher_product: input outside [0, 1] (the reference raises ValueError, reward_utils.py:237)",
               8: "non-finite observation or reward",
               16: "stepped after its episode ended with autoreset disabled (reset it with reset_mask first; the reference's "
-                  "SawyerXYZEnv.step raises ValueError past max_path_length)"}
+                  "SawyerXYZEnv.step raises ValueError past max_path_length)",
+              32: "load_states: no saved state of the env's model at the requested index (the env was left unchanged)"}
 
     def faults(self):
         """Per-env MW_FAULT_* bits since the last call (cleared)."""

@@ -95,6 +95,19 @@ class StepPost:
             self.xp = xp
         return xp
 
+    def save_rows(self):
+        """A copy of every env's wrapper state, in the namespace it is in now (`load_rows` takes it back)."""
+        return {k: v.copy() if isinstance(v, np.ndarray) else v.clone() for k in self._STATE if (v := getattr(self, k)) is not None}
+
+    def load_rows(self, rows, mask, src):
+        """Env e's wrapper state becomes row `src[e]` of `rows` (a `save_rows` result) where `mask[e]`.  `mask` (bool [N]) and
+        `src` (integer [N], in range) are numpy arrays or device tensors; the state moves to their namespace."""
+        xp = self._use(mask)
+        for k, v in rows.items():
+            if isinstance(v, np.ndarray) != (xp is _NUMPY):
+                v = xp.take(v)
+            setattr(self, k, xp.where(mask if v.ndim == 1 else mask[:, None], v[src], getattr(self, k)))
+
     @staticmethod
     def _merge(xp, mean, var, count, x):
         """N independent copies of gymnasium's RunningMeanStd.update (wrappers/utils.py), each fed one sample: the

@@ -29,7 +29,7 @@ import numpy as np
 
 from . import _gym
 from .benchmarks import Task, reference_env_id
-from .engine import ENVSTATE_DTYPE, INFO_KEYS, MAXDOF, MAXNQ, Engine, expert_actions
+from .engine import ENVSTATE_DTYPE, INFO_KEYS, MAXDOF, MAXNQ, NCONV, Engine, expert_actions
 from .getters import STATE_ATTRS, STATE_CALLS, StateGetters, _quat2mat  # noqa: F401  (_quat2mat: still importable from here)
 from .tasks import TASK_IDS, TASKS
 
@@ -116,6 +116,30 @@ class _SubEnv:
             self.current_task = self.next_task()
 
 
+_ENDED_WORD = ENVSTATE_DTYPE.fields["ended"][1] // 4       # the ended mark's float32 word in a 512-byte state record
+
+
+class EnvStates:
+    """Every env's complete state as `MetaWorldVecEnv.save_states` saved it, on the device; only the env that saved it can
+    load it (`load_states`, `load_states_torch`).  Row e is env e's state at the save; a row that was not selected then
+    holds no state (model id -1), and loading it fails like a model mismatch.
+    * `records` uint8 [N, 512], `model` int32 [N], `hints` float32 [N, NCONV, 4]: the engine's state records (the ended
+      mark of NEXT_STEP / DISABLED included), model slots and separating-axis hints;
+    * `raw`: float32 [N, 39], each env's last base observation; `obs`: the last observation returned to the caller
+      (a numpy array when the last call was the numpy `reset` / `step`, else a device tensor);
+    * `post`: the optional wrappers' per-env rows (`StepPost.save_rows`);
+    * `ep_len`, `tasks`: the host mirrors of the episode lengths and the running tasks."""
+
+    def __init__(self, owner, records, model, hints, raw, obs, post, ep_len, tasks):
+        self.owner, self.records, self.model, self.hints = owner, records, model, hints
+        self.raw, self.obs, self.post, self.ep_len, self.tasks = raw, obs, post, ep_len, tasks
+
+    def ended(self):
+        """bool [N] device tensor: the rows saved between a terminal step and its restart."""
+        import torch
+        return self.records.view(torch.float32)[:, _ENDED_WORD] != 0
+
+
 class MetaWorldVecEnv(_gym.VectorEnvBase):
     metadata = {"render_modes": [], "autoreset_mode": "same_step"}
 
@@ -166,7 +190,8 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             if rep:       # replicas are an extension (the reference has one sub-env per id): keep their ids distinct
                 eid += f".r{rep}"
             self.sub.append(_SubEnv(env_names[t_i], tasks_per_env[t_i], s, task_select != "random", eid))
-        self.engine.set_envs([self._slot[e % n_types] for e in range(num_envs)])
+        self._env_model = np.array([self._slot[e % n_types] for e in range(num_envs)], dtype=np.int32)   # env -> model slot
+        self.engine.set_envs(self._env_model)
         self._getters = StateGetters(self.engine, [s.task_name for s in self.sub])
         self._set_engine_options()
         if self.autoreset_mode != "SameStep":
@@ -195,6 +220,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self.d_final_obs = self.d_obs.clone()
         self.d_env_obs = self.d_obs.clone()            # observe_torch's output
         self.d_all = torch.ones(N, dtype=torch.bool, device=dev)
+        self.d_env_model = torch.from_numpy(self._env_model).to(dev)   # load_states_torch's check
         # the numpy API's outputs: the 39 columns k_step writes, packed (stride 39): the constant one-hot columns never cross
         # the bus, and the host converts a contiguous [N, 39] block
         self.d_obs39 = torch.zeros(N, 39, device=dev)
@@ -726,6 +752,127 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self.engine.observe(self._device_mask(env_mask), self.d_env_obs)
         return self.d_env_obs.cpu().numpy().astype(np.float64)
 
+    # ------------------------------------------------------------------ saved states (save, restore and fork on the device)
+    # A loaded env continues bit for bit as its source would have, up to the end of the current episode, in every autoreset
+    # mode.  The task-selection streams (host RNGs, the pending draw, the device sampler's key) are not part of a state:
+    # each env keeps its own, and `get_checkpoint` saves them.  Across a restart the replay is exact when the env draws
+    # the same snapshot as its source: always with the device sampler and `src` = identity (it keys on seed, env and
+    # the restored episode counter), and whenever `sample_tasks_on_reset` is False.  Fault bits, counters, profiles and
+    # the launch order are not part of a state.
+    def save_states(self, env_mask=None):
+        """An `EnvStates` with the complete state of every env with `env_mask` set (numpy or device bool [num_envs]; None =
+        all), without host synchronisation (with a numpy mask: one upload)."""
+        self._check_started("save_states")
+        t, N = self.torch, self.num_envs
+        mask = self._torch_mask(env_mask) if isinstance(env_mask, t.Tensor) else self._device_mask(env_mask)
+        records = t.zeros(N, 512, dtype=t.uint8, device=self.device)
+        model = t.full((N,), -1, dtype=t.int32, device=self.device)
+        hints = t.zeros(N, NCONV, 4, dtype=t.float32, device=self.device)
+        self.engine.save_states(records, model, hints, None if env_mask is None else mask)
+        if self._last_obs is not None:
+            obs = self._last_obs.copy()
+        else:
+            obs = (self._d_last_obs if self.post.active else self.d_obs).clone()
+        return EnvStates(self, records, model, hints, self._d_raw[:, :39].clone(), obs,
+                         self.post.save_rows() if self.post.active else None, self._ep_len.copy(),
+                         [s.current_task for s in self.sub])
+
+    def _check_states(self, states, what):
+        self._check_started(what)
+        if not isinstance(states, EnvStates) or states.owner is not self:
+            raise ValueError(f"{what}: the states were saved by another env (snapshot ids are engine-local)")
+
+    def _restore_mirrors(self, rows, ep_len, tasks, ended):
+        """The host mirrors of envs `rows` as a saved state has them: episode lengths, running tasks and (unless `ended` is
+        None) ended marks."""
+        self._ep_len[rows] = ep_len
+        for e, tk in zip(rows, tasks):
+            self.sub[e].current_task = tk
+        if ended is not None:
+            self._sync_ended_to_host()
+            self._ended[rows] = ended
+
+    def load_states(self, states, env_mask=None, src=None):
+        """Env e with `env_mask[e]` set (numpy bool [num_envs]; None = all) takes row `src[e]` (numpy integers [num_envs];
+        None = row e) of `states`, which this env saved.  A source row out of range, unsaved or of another model raises
+        ValueError before anything changes.  Returns the observations as `reset(options={"reset_mask": ...})` does: the
+        loaded envs' saved last observation, the other envs' last one.  Sub-envs that do not re-sample their task on
+        reset continue with the loaded task after the episode; the others keep their own task streams."""
+        self._check_states(states, "load_states")
+        N = self.num_envs
+        mask = np.ones(N, dtype=bool) if env_mask is None else np.asarray(env_mask)
+        if mask.shape != (N,) or mask.dtype != np.bool_:
+            raise ValueError(f"env_mask must be a numpy bool array of shape ({N},), got {mask.dtype} {mask.shape}")
+        src = np.arange(N) if src is None else np.asarray(src)
+        if src.shape != (N,) or src.dtype.kind not in "iu":
+            raise ValueError(f"src must be a numpy integer array of shape ({N},)")
+        src = np.where(mask, src, np.arange(N))         # unmasked rows: never read, kept in range for the row gathers below
+        rows = np.nonzero(mask)[0]
+        s = src[rows]
+        bad = rows[(s < 0) | (s >= N)]
+        if not len(bad):
+            bad = rows[states.model.cpu().numpy()[s] != self._env_model[rows]]
+        if len(bad):
+            raise ValueError(f"load_states: env(s) {bad.tolist()[:8]} have no saved state of their model at the given src")
+        t = self.torch
+        d_mask = t.from_numpy(mask).to(self.device)
+        d_src = t.from_numpy(src.astype(np.int32)).to(self.device)
+        self.engine.load_states(states.records, states.model, states.hints, d_mask, d_src)
+        self._restore_mirrors(rows, states.ep_len[s], [states.tasks[i] for i in s], states.ended().cpu().numpy()[s])
+        for e in rows:
+            if not self.sub[e].sample_tasks_on_reset:
+                self._draw_pending(e)
+        self._push_next()
+        self._d_raw[:, :39] = t.where(d_mask[:, None], states.raw[d_src.long()], self._d_raw[:, :39])
+        saved = states.obs if isinstance(states.obs, np.ndarray) else states.obs.cpu().numpy()
+        obs = (self._last_obs if self._last_obs is not None else self._last_obs_device().cpu().numpy()).astype(self.obs_dtype)
+        obs[rows] = saved[s]
+        if self.post.active:
+            self.post.load_rows(states.post, mask, src)
+        self._last_obs = obs
+        return obs
+
+    def _last_obs_device(self):
+        """What the last call returned, as a device tensor."""
+        if self._last_obs is not None:
+            return self.torch.from_numpy(np.asarray(self._last_obs, dtype=np.float32)).to(self.device)
+        return self._d_last_obs if self.post.active else self.d_obs
+
+    def load_states_torch(self, states, env_mask=None, src=None):
+        """`load_states` from device tensors, without host synchronisation: `env_mask` a bool tensor [num_envs] or None (all),
+        `src` an integer tensor [num_envs] or None (row e).  An env whose source row is out of range, unsaved or of another
+        model is left unchanged and gets fault bit 32 (`engine.raise_on_faults()` raises ValueError).  The host mirrors
+        (episode lengths, running tasks) are left as they are, as `step_torch` leaves them.  Returns the observations as
+        `reset_torch(mask)` does: the loaded envs' saved last observation, the other envs' last one."""
+        self._check_states(states, "load_states_torch")
+        t, N = self.torch, self.num_envs
+        mask = self._torch_mask(env_mask)
+        if src is None:
+            src = t.arange(N, device=self.device)
+        elif not (isinstance(src, t.Tensor) and src.device == self.device and not src.is_floating_point()
+                  and tuple(src.shape) == (N,)):
+            raise ValueError(f"src must be an integer tensor of shape ({N},) on {self.device}")
+        src = src.long()
+        sc = src.clamp(0, N - 1)
+        ok = mask & (src >= 0) & (src < N) & (states.model[sc] == self.d_env_model)    # the check of k_load_states
+        self.engine.load_states(states.records, states.model, states.hints, None if env_mask is None else mask,
+                                src.to(t.int32))
+        if self.autoreset_mode != "SameStep":
+            self._sync_ended_to_device()
+            self.d_ended.copy_(t.where(ok, states.ended()[sc], self.d_ended))
+        self._d_raw[:, :39] = t.where(ok[:, None], states.raw[sc], self._d_raw[:, :39])
+        saved = states.obs
+        if isinstance(saved, np.ndarray):          # saved right after a numpy call
+            saved = t.from_numpy(saved.astype(np.float32)).to(self.device)
+        out = t.where(ok[:, None], saved[sc], self._last_obs_device())
+        if self.post.active:
+            self.post.load_rows(states.post, ok, sc)
+        else:
+            self.d_obs.copy_(out)
+            out = self.d_obs
+        self._last_obs, self._d_last_obs = None, out
+        return out
+
     # ------------------------------------------------------------------ state accessors (SawyerXYZEnv / MujocoEnv getters)
     def query_torch(self, env_mask=None, bodies=(), sites=(), geoms=(), touching=False):
         """Read-only accessors of every env's current state (envs with `env_mask` set; bool tensor [num_envs], None =
@@ -908,6 +1055,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             new_tasks += [_deserialize_task(t) for t in ck["tasks"]]
         self._ensure_snapshots(new_tasks)
         st = None
+        rows, lens, cur = [], [], []
         for e, (s, ck) in enumerate(zip(self.sub, mine)):
             s.pending, s._pre = None, None
             s.tasks = [_deserialize_task(t) for t in ck["tasks"]]
@@ -924,12 +1072,14 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             s.space_rng["goal_space"].bit_generator.state = ers["goal_space_rng_state"]
             ext = ck.get("mw_b200")
             if ext is not None:
-                self._ep_len[e] = ext["ep_len"]
-                s.current_task = None if ext["current_task"] is None else _deserialize_task(ext["current_task"])
+                rows.append(e); lens.append(ext["ep_len"])
+                cur.append(None if ext["current_task"] is None else _deserialize_task(ext["current_task"]))
                 if "state" in ext:
                     if st is None:
                         st = self.engine.get_state()
                     st[e] = np.frombuffer(base64.b64decode(ext["state"]), dtype=ENVSTATE_DTYPE)[0]
+        # (the ended mark: a run stopped between a terminal step and its restart)
+        self._restore_mirrors(rows, lens, cur, None if st is None else st["ended"][rows] != 0)
         if st is not None:
             # snapshot ids are engine-local: re-point every restored record at this engine's id for the same task
             for e, s in enumerate(self.sub):
@@ -938,7 +1088,6 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
                     st[e]["snapshot"] = self._snap(s.current_task)
             self.engine.set_state(st)
             self._needs_reset = False
-            self._ended, self._ended_on_device = st["ended"] != 0, False      # a run stopped between a terminal step and its restart
         if not self._needs_reset:
             for e, s in enumerate(self.sub):
                 if s.current_task is None:
