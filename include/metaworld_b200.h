@@ -96,6 +96,25 @@ int mw_set_autoreset_mode(mw_engine*, int mode);
  * snapshot_ids DEV [n_envs] or NULL, obs DEV float [n_envs, obs_stride].                                             */
 int mw_reset_masked(mw_engine*, const unsigned char* mask, const int* snapshot_ids, float* obs, int obs_stride, void* stream);
 
+/* Episodes at goals outside the snapshot table (SawyerXYZEnv._get_state_rand_vec with _freeze_rand_vec False,
+ * metaworld/sawyer_xyz_env.py:697-719: a new goal in every reset_model pass), without a table entry or a host round trip.
+ * mw_build_goal_rows runs, for every env with mask[i] != 0, the reference's reset() of that env's model with
+ * rand_vec_pass1[i] in the first reset_model pass and rand_vec[i] in the second (rand_vec_pass1 NULL: rand_vec in both) and
+ * writes the episode-start record to rows[i]: byte for byte the record mw_build_snapshots makes for the same (model,
+ * rand_vec, rand_vec_pass1, partially_observable) in the same library, except the snapshot field, which is -1.  A task
+ * whose vector is shorter than 6 reads the leading columns.  A masked env whose goal is not finite gets a row with a NaN
+ * observation.  Rows of unmasked envs are not written.  Launched over the engine's CTA table; the rows may be built by
+ * the float64 library's engine (same env table) and loaded by the float32 one: the record layout is the same.
+ * mw_reset_rows restarts every env with mask[i] != 0 from rows[i] as mw_reset_masked does from a table row: its episode
+ * counter advances by one, path length and return are 0, the ended mark is cleared, the snapshot field is -1 and obs row
+ * i is written.  An env whose row has a non-finite goal (_target_pos) or observation is left unchanged and gets
+ * MW_FAULT_BAD_GOAL.  Neither call allocates or synchronises.
+ *   mask DEV u8 [n_envs]; rand_vec, rand_vec_pass1 DEV f64 [n_envs, 6]; partially_observable DEV u8 [n_envs];
+ *   rows DEV [n_envs] 768-byte snapshot records (mw_sizeof_snapshot), owned by the caller; obs DEV f32 [n_envs, obs_stride]. */
+int mw_build_goal_rows(mw_engine*, const unsigned char* mask, const double* rand_vec, const double* rand_vec_pass1,
+                       const unsigned char* partially_observable, void* rows, void* stream);
+int mw_reset_rows(mw_engine*, const unsigned char* mask, const void* rows, float* obs, int obs_stride, void* stream);
+
 /* SawyerXYZEnv.evaluate_state(obs, action) (metaworld/sawyer_xyz_env.py:644-656 -> the task's evaluate_state /
  * compute_reward): reward and info of every env's CURRENT physics state for caller-supplied observations and actions.
  * One forward pass (poses, contact forces for touching_object), no state change.  actions DEV [n,4], obs DEV
@@ -176,7 +195,9 @@ int mw_expert_actions(const int* task_ids, const float* obs, int obs_stride, int
  *  16 MW_FAULT_STEP_AFTER_END  DISABLED autoreset: stepped after its episode ended, before mw_reset_masked (gymnasium's
  *                              SyncVectorEnv asserts; SawyerXYZEnv.step raises past max_path_length).  API misuse.
  *  32 MW_FAULT_BAD_LOAD    mw_load_states: the env's source record is out of range or holds another model slot; the env
- *                          was left unchanged.  API misuse.                                                          */
+ *                          was left unchanged.  API misuse.
+ *  64 MW_FAULT_BAD_GOAL    mw_reset_rows: the env's row has a non-finite goal or observation; the env was left
+ *                          unchanged.  API misuse.                                                                    */
 int mw_get_faults(mw_engine*, int* out);
 
 /* options: max_episode_steps (TimeLimit), terminate_on_success (0/1), device sampler seed */

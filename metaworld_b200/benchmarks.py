@@ -210,8 +210,13 @@ def make_tasks(env_names, partially_observable: bool, seed=None, n_goals=N_GOALS
         if len(np.unique(np.array(vecs), axis=0)) != n_goals:
             raise AssertionError(f"Only generated {len(np.unique(np.array(vecs), axis=0))} unique goals, not {n_goals}")
         for v in vecs:
-            tasks.append(Task(name, pickle.dumps(dict(rand_vec=v, env_cls=_RefClass(REFERENCE_CLASS[name]), partially_observable=partially_observable))))
+            tasks.append(make_task(name, v, partially_observable))
     return tasks
+
+
+def make_task(name, rand_vec, partially_observable: bool):
+    """The reference's ``Task`` of env class `name` with goal vector `rand_vec` (metaworld/__init__.py:171)."""
+    return Task(name, pickle.dumps(dict(rand_vec=rand_vec, env_cls=_RefClass(REFERENCE_CLASS[name]), partially_observable=partially_observable)))
 
 
 class EnvClass:

@@ -348,15 +348,13 @@ k_step(EngineDev e, const int* __restrict__ block_order, BlockTable bt, const fl
   }
 }
 
-// builds episode-start snapshots: exact reset() sequence of the reference (reset_model, mj_resetData, reset_model)
-__global__ void __launch_bounds__(BLOCK_THREADS, 1)
-k_snapshot(EngineDev e, BlockTable bt, const double* __restrict__ rand_vec, const double* __restrict__ rand_vec_pass1, const unsigned char* __restrict__ partial, int snap_base) {
-  CtaWarp cw;
-  if (!cta_enter(e, bt, blockIdx.x, cw)) return;
+// The reference's reset() (reset_model, mj_resetData, reset_model) of the warp's model with rand_vec rv1 in the first
+// reset_model pass and rv2 in the second (an unfrozen rand_vec draws once per pass): leaves the episode-start record in
+// ws->es, its snapshot field unset, and the reset observation in ws->obs.  Every warp of the CTA runs it (phase barriers).
+// Shared by k_snapshot and k_goal_rows, so that a goal row is the snapshot of the same goal byte for byte.
+DEV void reset_episode(const EngineDev& e, const CtaWarp& cw, const double* rv1, const double* rv2, bool partial) {
   BlockShared* bs = cw.bs; WarpShared* ws = cw.ws; WarpScratch* w = cw.w; const MwModel* m = cw.m;
-  const int lane = cw.lane, item = cw.env;
-  const double* rv2 = rand_vec + 6 * item;
-  const double* rv1 = rand_vec_pass1 ? rand_vec_pass1 + 6 * item : rv2;   // an unfrozen rand_vec draws once per reset_model pass
+  const int lane = cw.lane;
   real act[4] = {0, 0, 0, 0};
   TaskCtx c = task_ctx(e, cw, act);
   for (int i = lane; i < 128; i += 32) ((float*)&ws->es)[i] = 0.f;
@@ -385,18 +383,77 @@ k_snapshot(EngineDev e, BlockTable bt, const double* __restrict__ rand_vec, cons
     SYNCW();
   }
   if (lane == 0) {
-    ws->es.partially_observable = partial[item] ? 1.f : 0.f;
+    ws->es.partially_observable = partial ? 1.f : 0.f;
     make_obs(c, ws->obs, false);                       // _get_obs() of pass 2, not clipped
     for (int i = 0; i < 18; i++) { ws->obs[18 + i] = ws->obs[i]; }   // reset(): obs[18:36] = obs[:18]  (:679-680)
-    ws->es.path_len = 0.f; ws->es.episode = 0.f; ws->es.ep_return = 0.f; ws->es.snapshot = (float)(snap_base + item);
+    ws->es.path_len = 0.f; ws->es.episode = 0.f; ws->es.ep_return = 0.f;
     ws->es.gripper_ctrl = -1.f;                        // _reset_hand leaves ctrl = [-1, 1]
   }
   SYNCW();
   if (lane < 3) ws->es.shift[lane] = (float)w->shift[lane];
   SYNCW();
-  MwSnapshot* sp = e.snaps + snap_base + item;
+}
+
+// the warp's reset_episode result with snapshot field `snapshot`, as the MwSnapshot record `sp`
+DEV void store_snapshot(WarpShared* ws, MwSnapshot* sp, float snapshot, int lane) {
+  if (lane == 0) ws->es.snapshot = snapshot;
+  SYNCW();
   store_env(ws, &sp->st, lane);
   for (int i = lane; i < 39; i += 32) sp->obs[i] = ws->obs[i];
+}
+
+// builds episode-start snapshots: exact reset() sequence of the reference (reset_model, mj_resetData, reset_model)
+__global__ void __launch_bounds__(BLOCK_THREADS, 1)
+k_snapshot(EngineDev e, BlockTable bt, const double* __restrict__ rand_vec, const double* __restrict__ rand_vec_pass1, const unsigned char* __restrict__ partial, int snap_base) {
+  CtaWarp cw;
+  if (!cta_enter(e, bt, blockIdx.x, cw)) return;
+  const int item = cw.env;
+  const double* rv2 = rand_vec + 6 * item;
+  reset_episode(e, cw, rand_vec_pass1 ? rand_vec_pass1 + 6 * item : rv2, rv2, partial[item] != 0);
+  store_snapshot(cw.ws, e.snaps + snap_base + item, (float)(snap_base + item), cw.lane);
+}
+
+// whether env's goal is finite in both passes (rand_vec_pass1 NULL: rand_vec in both)
+DEV bool goal_finite(const double* __restrict__ rand_vec, const double* __restrict__ rand_vec_pass1, int env) {
+  bool ok = true;
+  for (int i = 0; i < 6; i++) ok = ok && isfinite(rand_vec[6 * env + i]) && (!rand_vec_pass1 || isfinite(rand_vec_pass1[6 * env + i]));
+  return ok;
+}
+
+// Goal rows (mw_build_goal_rows) over the engine's CTA table: every env with mask[env] set gets the episode-start record
+// of its own goal in rows[env], snapshot field -1.  A CTA with no masked env leaves before its first barrier
+// (cta_has_masked).  In a CTA that stays, every warp runs reset_episode to meet the phase barriers: a warp without a goal
+// of its own (unmasked, or a non-finite goal) runs the goal of the CTA's first masked env with a finite one, the donor,
+// and discards the result; a masked env with a non-finite goal gets a NaN observation, which mw_reset_rows refuses.
+// When the CTA has no donor its warps write those NaN observations and leave without any physics.
+__global__ void __launch_bounds__(BLOCK_THREADS, 1)
+k_goal_rows(EngineDev e, BlockTable bt, const unsigned char* __restrict__ mask, const double* __restrict__ rand_vec,
+            const double* __restrict__ rand_vec_pass1, const unsigned char* __restrict__ partial, MwSnapshot* __restrict__ rows) {
+  if (!cta_has_masked(bt, blockIdx.x, mask)) return;
+  const int first = bt.start[blockIdx.x], count = bt.count[blockIdx.x];
+  int donor = -1;
+  for (int k = 0; k < count && donor < 0; k++) {
+    const int env = bt.perm[first + k];
+    if (mask[env] && goal_finite(rand_vec, rand_vec_pass1, env)) donor = env;
+  }
+  const float nan = __int_as_float(0x7fc00000);
+  if (donor < 0) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (warp >= count) return;
+    const int env = bt.perm[first + warp];
+    if (mask[env]) for (int i = lane; i < 39; i += 32) rows[env].obs[i] = nan;
+    return;
+  }
+  CtaWarp cw;
+  if (!cta_enter(e, bt, blockIdx.x, cw)) return;
+  const int env = cw.env, lane = cw.lane;
+  const bool own = mask[env] && goal_finite(rand_vec, rand_vec_pass1, env);
+  const int g = own ? env : donor;
+  const double* rv2 = rand_vec + 6 * g;
+  reset_episode(e, cw, rand_vec_pass1 ? rand_vec_pass1 + 6 * g : rv2, rv2, partial[g] != 0);
+  if (!mask[env]) return;                              // after the CTA's last barrier
+  if (own) store_snapshot(cw.ws, rows + env, -1.f, lane);
+  else for (int i = lane; i < 39; i += 32) rows[env].obs[i] = nan;
 }
 
 __global__ void k_reset(EngineDev e, int n, const int* __restrict__ env_ids, const int* __restrict__ snapshot_ids,
@@ -426,6 +483,32 @@ __global__ void k_reset_masked(EngineDev e, const unsigned char* __restrict__ ma
   __syncwarp();
   if (lane == 0) { e.state[env].episode = episode + 1.f; e.state[env].snapshot = (float)snap; }
   for (int i = lane; i < 39; i += 32) obs[(size_t)env * obs_stride + i] = sp->obs[i];
+}
+
+// mw_reset_rows, one warp per env: k_reset_masked from the caller's row rows[env] instead of a table row, with snapshot
+// field -1 and the counters of a fresh episode set here (a caller's row may hold anything there).  A row whose goal
+// (_target_pos) or observation is not finite leaves the env as it is and flags MW_FAULT_BAD_GOAL.
+__global__ void k_reset_rows(EngineDev e, const unsigned char* __restrict__ mask, const MwSnapshot* __restrict__ rows,
+                             float* __restrict__ obs, int obs_stride) {
+  const int env = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (env >= e.n_envs || !mask[env]) return;
+  const MwSnapshot* sp = rows + env;
+  const float o0 = sp->obs[lane], o1 = lane < 39 - 32 ? sp->obs[32 + lane] : 0.f, tg = lane < 3 ? sp->st.target[lane] : 0.f;
+  if (!__all_sync(0xffffffffu, isfinite(o0) && isfinite(o1) && isfinite(tg))) {
+    if (lane == 0) e.diag[3 * env + 2] |= MW_FAULT_BAD_GOAL;
+    return;
+  }
+  const float episode = e.state[env].episode;
+  float4 v = ((const float4*)&sp->st)[lane];
+  __syncwarp();                                        // every lane has read `episode` before the record is overwritten
+  ((float4*)(e.state + env))[lane] = v;
+  __syncwarp();
+  if (lane == 0) {
+    MwEnvState* s = e.state + env;
+    s->episode = episode + 1.f; s->snapshot = -1.f; s->path_len = 0.f; s->ep_return = 0.f; s->ended = 0.f;
+  }
+  obs[(size_t)env * obs_stride + lane] = o0;
+  if (lane < 39 - 32) obs[(size_t)env * obs_stride + 32 + lane] = o1;
 }
 
 __global__ void __launch_bounds__(BLOCK_THREADS, 1)
@@ -908,7 +991,7 @@ static int read_diag(const mw_engine* E, std::vector<int>& diag) {
   return 0;
 }
 
-// one warp per row (k_reset, k_reset_masked, k_set_physics, k_get_physics, k_save_states, k_load_states)
+// one warp per row (k_reset, k_reset_masked, k_reset_rows, k_set_physics, k_get_physics, k_save_states, k_load_states)
 #define ROW_THREADS 256
 static int row_blocks(int rows) { return (rows * 32 + ROW_THREADS - 1) / ROW_THREADS; }
 
@@ -969,6 +1052,7 @@ int mw_create(mw_engine** out, int device, int n_models, const void* models, con
   CK(cudaFuncSetAttribute(k_step<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_step<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_snapshot, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
+  CK(cudaFuncSetAttribute(k_goal_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_substeps, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_evaluate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_observe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
@@ -1067,6 +1151,24 @@ int mw_reset_masked(mw_engine* E, const unsigned char* mask, const int* snapshot
   if (!snapshot_ids && !E->d_goal_first.p) return fail(MW_ERR_STATE, "mw_reset_masked: no snapshot_ids and no goal sets for the device sampler");
   CK(cudaSetDevice(E->device));
   k_reset_masked<<<row_blocks(E->n_envs), ROW_THREADS, 0, (cudaStream_t)stream>>>(E->dev(), mask, snapshot_ids, obs, obs_stride);
+  return launched(E, 1);
+}
+
+int mw_build_goal_rows(mw_engine* E, const unsigned char* mask, const double* rand_vec, const double* rand_vec_pass1,
+                       const unsigned char* partial, void* rows, void* stream) {
+  if (!E || !E->d_state.p) return fail(MW_ERR_STATE, "mw_build_goal_rows: mw_set_envs not called");
+  if (!mask || !rand_vec || !partial || !rows) return fail(MW_ERR_ARG, "mw_build_goal_rows: bad arguments");
+  CK(cudaSetDevice(E->device));
+  k_goal_rows<<<E->blk.n_blocks, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), E->blocks(), mask, rand_vec, rand_vec_pass1,
+                                                                                    partial, (MwSnapshot*)rows);
+  return launched(E, 1);
+}
+
+int mw_reset_rows(mw_engine* E, const unsigned char* mask, const void* rows, float* obs, int obs_stride, void* stream) {
+  if (!E || !E->d_state.p) return fail(MW_ERR_STATE, "mw_reset_rows: mw_set_envs not called");
+  if (!mask || !rows || !obs || obs_stride < 39) return fail(MW_ERR_ARG, "mw_reset_rows: bad arguments");
+  CK(cudaSetDevice(E->device));
+  k_reset_rows<<<row_blocks(E->n_envs), ROW_THREADS, 0, (cudaStream_t)stream>>>(E->dev(), mask, (const MwSnapshot*)rows, obs, obs_stride);
   return launched(E, 1);
 }
 

@@ -53,6 +53,7 @@ enum { INFO_SUCCESS = 0, INFO_NEAR_OBJECT, INFO_GRASP_SUCCESS, INFO_GRASP_REWARD
 #define MW_FAULT_NONFINITE 8
 #define MW_FAULT_STEP_AFTER_END 16   // DISABLED autoreset: an env was stepped after its episode ended (API misuse, not a GPU fault)
 #define MW_FAULT_BAD_LOAD 32         // mw_load_states: no saved record of the env's model at the given index (API misuse)
+#define MW_FAULT_BAD_GOAL 64         // mw_reset_rows: the env's row has a non-finite goal or observation (API misuse)
 DEV real tol_long_tail_f(int* fault, real x, real lo, real hi, real margin) {
   if (lo > hi) *fault |= MW_FAULT_TOL_BOUNDS;
   if (margin < 0) *fault |= MW_FAULT_TOL_MARGIN;

@@ -58,6 +58,8 @@ def _load(path):
     L.mw_step.argtypes = [vp, vp, vp, ip, vp, vp, vp, vp, ip, vp, vp, vp, vp]
     L.mw_set_autoreset_mode.argtypes = [vp, ip]
     L.mw_reset_masked.argtypes = [vp, vp, vp, vp, ip, vp]
+    L.mw_build_goal_rows.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    L.mw_reset_rows.argtypes = [vp, vp, vp, vp, ip, vp]
     L.mw_set_options.argtypes = [vp, ip, ip, C.c_ulonglong]
     L.mw_set_goal_sets.argtypes = [vp, vp, vp]
     L.mw_get_state.argtypes = [vp, vp]
@@ -184,6 +186,7 @@ class Engine:
         _ck(lib().mw_create(C.byref(self.h), device, len(self.specs), models.ctypes.data, tcs.ctypes.data, ptrs,
                             nmv.ctypes.data))
         self.h64 = None
+        self._h64_env_model = None   # the env table mw_set_envs last gave h64 (build_goal_rows)
         self.n_envs = 0
         self._query_tables = {}      # device copies of the mw_query tables, by frame list / geom list
 
@@ -228,21 +231,55 @@ class Engine:
         po = np.ascontiguousarray(partially_observable, dtype=np.uint8)
         ids = np.zeros(len(mi), dtype=np.int32)
         if precise is None:
-            precise = os.environ.get("MW_B200_SNAPSHOT_F32", "0") != "1" and SO_PATH != SO64_PATH
+            precise = self._precise()
         if not precise:
             _ck(lib().mw_build_snapshots(self.h, len(mi), mi.ctypes.data, rv.ctypes.data, p1, po.ctypes.data, ids.ctypes.data))
             return ids
         L = lib64()
-        if self.h64 is None:
-            device, nm, models, tcs, ptrs, nmv = self._create_args
-            self.h64 = C.c_void_p()
-            _ck(L.mw_create(C.byref(self.h64), device, nm, models.ctypes.data, tcs.ctypes.data, ptrs, nmv.ctypes.data), L)
+        self._engine64()
         first = L.mw_num_snapshots(self.h64)
         _ck(L.mw_build_snapshots(self.h64, len(mi), mi.ctypes.data, rv.ctypes.data, p1, po.ctypes.data, None), L)
         rec = np.zeros(len(mi), dtype=SNAPSHOT_DTYPE)
         _ck(L.mw_get_snapshots(self.h64, first, len(mi), rec.ctypes.data), L)
         _ck(lib().mw_append_snapshots(self.h, len(mi), rec.ctypes.data, ids.ctypes.data))
         return ids
+
+    @staticmethod
+    def _precise():
+        """Whether episode starts are computed by the float64 build (the default; MW_B200_SNAPSHOT_F32=1 turns it off)."""
+        return os.environ.get("MW_B200_SNAPSHOT_F32", "0") != "1" and SO_PATH != SO64_PATH
+
+    def _engine64(self):
+        """The float64 build's engine over the same models (created on first use)."""
+        if self.h64 is None:
+            device, nm, models, tcs, ptrs, nmv = self._create_args
+            h = C.c_void_p()
+            _ck(lib64().mw_create(C.byref(h), device, nm, models.ctypes.data, tcs.ctypes.data, ptrs, nmv.ctypes.data), lib64())
+            self.h64 = h
+        return self.h64
+
+    def build_goal_rows(self, mask, rand_vec, rand_vec_pass1, partial, rows):
+        """Episode-start records of new goals (mw_build_goal_rows): row e of `rows` (uint8 device tensor [n_envs, 768],
+        contiguous) becomes, for every env e with `mask` set (bool device tensor [n_envs]), the snapshot that
+        `build_snapshots` would make for its model with `rand_vec[e]` (float64 device tensor [n_envs, 6]; pass 1:
+        `rand_vec_pass1[e]`, None = the same) and observability `partial[e]` (uint8 device tensor [n_envs]), with snapshot
+        field -1.  Precise mode (the default, as for `build_snapshots`) runs it on the float64 build's engine, given this
+        engine's env table, on the same stream; `reset_rows` then reads the rows in place."""
+        args = (self._p(mask), self._p(rand_vec), self._p(rand_vec_pass1), self._p(partial), self._p(rows), self._stream())
+        if not self._precise():
+            _ck(lib().mw_build_goal_rows(self.h, *args))
+            return
+        h = self._engine64()
+        if self._h64_env_model is not self.env_model:
+            _ck(lib64().mw_set_envs(h, len(self.env_model), self.env_model.ctypes.data), lib64())
+            self._h64_env_model = self.env_model
+        _ck(lib64().mw_build_goal_rows(h, *args), lib64())
+
+    def reset_rows(self, mask, rows, obs):
+        """Restarts the envs with `mask` set from their rows of `rows` (a `build_goal_rows` result) as `reset_masked` does
+        from a snapshot, with snapshot field -1; writes those rows of `obs`.  A row with a non-finite goal or observation
+        leaves its env unchanged and sets fault bit 64 (mw_reset_rows)."""
+        _ck(lib().mw_reset_rows(self.h, self._p(mask), self._p(rows), self._p(obs), obs.stride(0), self._stream()))
 
     def get_snapshots(self, first=0, n=None):
         n = lib().mw_num_snapshots(self.h) - first if n is None else n
@@ -349,7 +386,8 @@ class Engine:
               8: "non-finite observation or reward",
               16: "stepped after its episode ended with autoreset disabled (reset it with reset_mask first; the reference's "
                   "SawyerXYZEnv.step raises ValueError past max_path_length)",
-              32: "load_states: no saved state of the env's model at the requested index (the env was left unchanged)"}
+              32: "load_states: no saved state of the env's model at the requested index (the env was left unchanged)",
+              64: "reset_rows: the env's goal row has a non-finite goal or observation (the env was left unchanged)"}
 
     def faults(self):
         """Per-env MW_FAULT_* bits since the last call (cleared)."""

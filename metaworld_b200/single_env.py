@@ -72,6 +72,7 @@ class SawyerXYZEnvB200:
         self._set_task_called = False
         self._last_rand_vec = None
         self._freeze_rand_vec = True
+        self.seeded_rand_vec = False                 # unfrozen draws from self.np_random instead of np.random (:702-710)
         self._snap_cache: dict = {}
         self._snap_id = None
         self._did_reset = False
@@ -86,6 +87,7 @@ class SawyerXYZEnvB200:
         self.d_term = t.zeros(1, dtype=t.uint8, device=dev); self.d_trunc = t.zeros(1, dtype=t.uint8, device=dev)
         self.d_info = t.zeros(1, 9, device=dev); self.d_fobs = t.zeros(1, 39, device=dev); self.d_finfo = t.zeros(1, 8, device=dev)
         self.d_act = t.zeros(1, 4, device=dev); self.d_sid = t.zeros(1, dtype=t.int32, device=dev)
+        self._goal_bufs = None       # (goal row, goal vectors, observability, mask) of the unfrozen reset, made on first use
         self._last_stable_obs = None
 
     # ---- spaces (sawyer_xyz_env.py:529-577): recomputed when observability changes, like the cached_property there
@@ -128,15 +130,39 @@ class SawyerXYZEnvB200:
 
     def reset(self, seed=None, options=None, _pass1=None):
         """sawyer_xyz_env.py:664-682 (`seed` / `options` ignored there too).  The double-pass reset is evaluated by the
-        device once per distinct (rand_vec, observability) and cached as an episode-start snapshot."""
-        assert self._last_rand_vec is not None, "set_task must be called before reset (the reference asserts in _get_state_rand_vec)"
+        device once per distinct (rand_vec, observability) and cached as an episode-start snapshot.  With
+        `_freeze_rand_vec` False each reset_model pass draws a new goal as `_get_state_rand_vec` does (:697-719), from
+        np.random or, when `seeded_rand_vec`, from `np_random`; `_last_rand_vec` is the second pass's, and the episode
+        starts from a goal row built on the device, which the snapshot table never holds."""
         self.curr_path_length = 0
-        self._snap_id = self._snapshot(_pass1)
-        self.d_sid[0] = self._snap_id
-        self.engine.reset(self.d_sid, self.d_obs)
+        if not self._freeze_rand_vec:
+            self._reset_unfrozen()
+        else:
+            assert self._last_rand_vec is not None, "set_task must be called before reset (the reference asserts in _get_state_rand_vec)"
+            self._snap_id = self._snapshot(_pass1)
+            self.d_sid[0] = self._snap_id
+            self.engine.reset(self.d_sid, self.d_obs)
         self._did_reset = True
         self._goal_site_written = self.env_name == "shelf-place-v3"
         return self.d_obs[0].cpu().numpy().astype(np.float64), {}
+
+    def _reset_unfrozen(self):
+        from .benchmarks import draw_rand_vec
+
+        src = self.np_random if self.seeded_rand_vec else np.random
+        first = draw_rand_vec(self.spec_, src)                 # reset_model pass 1
+        self._last_rand_vec = draw_rand_vec(self.spec_, src)   # pass 2
+        t, dev = self.torch, self.engine.device
+        if self._goal_bufs is None:
+            self._goal_bufs = (t.zeros(1, 768, dtype=t.uint8, device=dev), t.zeros(2, 1, 6, dtype=t.float64, device=dev),
+                               t.zeros(1, dtype=t.uint8, device=dev), t.ones(1, dtype=t.bool, device=dev))
+        row, rv, po, mask = self._goal_bufs
+        v = np.zeros((2, 1, 6))
+        v[0, 0, : first.size], v[1, 0, : self._last_rand_vec.size] = first, self._last_rand_vec
+        rv.copy_(t.from_numpy(v))
+        po.fill_(int(self._partially_observable))
+        self.engine.build_goal_rows(mask, rv[1], rv[0], po, row)
+        self.engine.reset_rows(mask, row, self.d_obs)
 
     @_assert_task_is_set
     def step(self, action):

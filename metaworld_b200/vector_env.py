@@ -28,8 +28,8 @@ import base64
 import numpy as np
 
 from . import _gym
-from .benchmarks import Task, reference_env_id
-from .engine import ENVSTATE_DTYPE, INFO_KEYS, MAXDOF, MAXNQ, NCONV, Engine, expert_actions
+from .benchmarks import Task, draw_rand_vec, make_task, reference_env_id
+from .engine import ENVSTATE_DTYPE, INFO_KEYS, MAXDOF, MAXNQ, NCONV, SNAPSHOT_DTYPE, Engine, expert_actions
 from .getters import STATE_ATTRS, STATE_CALLS, StateGetters, _quat2mat  # noqa: F401  (_quat2mat: still importable from here)
 from .tasks import TASK_IDS, TASKS
 
@@ -117,6 +117,9 @@ class _SubEnv:
 
 
 _ENDED_WORD = ENVSTATE_DTYPE.fields["ended"][1] // 4       # the ended mark's float32 word in a 512-byte state record
+# the float32 words of a 768-byte goal row (engine.build_goal_rows) that mw_reset_rows checks: _target_pos and the observation
+_ROW_TARGET = ENVSTATE_DTYPE.fields["target"][1] // 4
+_ROW_OBS = SNAPSHOT_DTYPE.fields["obs"][1] // 4
 
 
 class EnvStates:
@@ -128,11 +131,12 @@ class EnvStates:
     * `raw`: float32 [N, 39], each env's last base observation; `obs`: the last observation returned to the caller
       (a numpy array when the last call was the numpy `reset` / `step`, else a device tensor);
     * `post`: the optional wrappers' per-env rows (`StepPost.save_rows`);
-    * `ep_len`, `tasks`: the host mirrors of the episode lengths and the running tasks."""
+    * `ep_len`, `tasks`: the host mirrors of the episode lengths and the running tasks;
+    * `goal`: float64 [N, 6], the running goals of the envs on a `reset_goals` goal (None before the first such reset)."""
 
-    def __init__(self, owner, records, model, hints, raw, obs, post, ep_len, tasks):
+    def __init__(self, owner, records, model, hints, raw, obs, post, ep_len, tasks, goal):
         self.owner, self.records, self.model, self.hints = owner, records, model, hints
-        self.raw, self.obs, self.post, self.ep_len, self.tasks = raw, obs, post, ep_len, tasks
+        self.raw, self.obs, self.post, self.ep_len, self.tasks, self.goal = raw, obs, post, ep_len, tasks, goal
 
     def ended(self):
         """bool [N] device tensor: the rows saved between a terminal step and its restart."""
@@ -221,6 +225,10 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self.d_env_obs = self.d_obs.clone()            # observe_torch's output
         self.d_all = torch.ones(N, dtype=torch.bool, device=dev)
         self.d_env_model = torch.from_numpy(self._env_model).to(dev)   # load_states_torch's check
+        # reset_goals: each env's observability (constant over its task list) and, allocated on first use, the goal rows,
+        # that flag on the device and the running goal of every env whose record has snapshot id -1
+        self._partial = np.array([bool(s.tasks[0].unpack()["partially_observable"]) for s in self.sub])
+        self._goal_bufs = None
         # the numpy API's outputs: the 39 columns k_step writes, packed (stride 39): the constant one-hot columns never cross
         # the bus, and the host converts a contiguous [N, 39] block
         self.d_obs39 = torch.zeros(N, 39, device=dev)
@@ -626,6 +634,12 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         if self._last_obs is not None and not self.post.active:      # the previous call was the numpy `reset` / `step`
             self.d_obs.copy_(t.from_numpy(np.asarray(self._last_obs, dtype=np.float32)))
         self.engine.reset_masked(mask, self.d_obs, None if self._device_sampler else self.d_next)
+        return self._restarted(mask)
+
+    def _restarted(self, mask):
+        """The bookkeeping of a masked restart into `d_obs` (bool device tensor `mask`): base rows, ended marks, the
+        optional wrappers' reset; returns the observations as `reset_torch(mask)` does."""
+        t = self.torch
         self._merge_raw_rows(mask)
         self._sync_ended_to_device()
         self.d_ended &= ~mask
@@ -775,7 +789,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             obs = (self._d_last_obs if self.post.active else self.d_obs).clone()
         return EnvStates(self, records, model, hints, self._d_raw[:, :39].clone(), obs,
                          self.post.save_rows() if self.post.active else None, self._ep_len.copy(),
-                         [s.current_task for s in self.sub])
+                         [s.current_task for s in self.sub], None if self._goal_bufs is None else self._goal_bufs[2].clone())
 
     def _check_states(self, states, what):
         self._check_started(what)
@@ -824,6 +838,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
                 self._draw_pending(e)
         self._push_next()
         self._d_raw[:, :39] = t.where(d_mask[:, None], states.raw[d_src.long()], self._d_raw[:, :39])
+        self._load_goals(states, d_mask, d_src.long())
         saved = states.obs if isinstance(states.obs, np.ndarray) else states.obs.cpu().numpy()
         obs = (self._last_obs if self._last_obs is not None else self._last_obs_device().cpu().numpy()).astype(self.obs_dtype)
         obs[rows] = saved[s]
@@ -861,6 +876,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             self._sync_ended_to_device()
             self.d_ended.copy_(t.where(ok, states.ended()[sc], self.d_ended))
         self._d_raw[:, :39] = t.where(ok[:, None], states.raw[sc], self._d_raw[:, :39])
+        self._load_goals(states, ok, sc)
         saved = states.obs
         if isinstance(saved, np.ndarray):          # saved right after a numpy call
             saved = t.from_numpy(saved.astype(np.float32)).to(self.device)
@@ -872,6 +888,108 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             out = self.d_obs
         self._last_obs, self._d_last_obs = None, out
         return out
+
+    def _load_goals(self, states, mask, src):
+        """The running goals of a load: env e takes row `src[e]` of the saved goal table where `mask[e]` (device tensors)."""
+        if states.goal is not None:
+            goal = self._goal_buffers()[2]
+            goal.copy_(self.torch.where(mask[:, None], states.goal[src], goal))
+
+    # ------------------------------------------------------------------ episodes at new goals (unfrozen rand_vec)
+    # `reset_goals_torch(g, m)` is `engine.reset_masked(m, obs, ids)` with `ids` the snapshots of the goals `g`, except that
+    # no snapshot is built or stored and the records' snapshot id is -1.  No task-selection draw is consumed: the pending
+    # draw stays pending, and the device sampler draws for the next episode as for any other.  The goal an env runs on is
+    # part of its state until its next reset: `get_attr("_last_rand_vec")`, `save_states` / `load_states` and the
+    # checkpoints carry it.
+    def _goal_buffers(self):
+        """(goal rows uint8 [N, 768], observability uint8 [N], running goals float64 [N, 6]) on the device."""
+        if self._goal_bufs is None:
+            t, N = self.torch, self.num_envs
+            self._goal_bufs = (t.zeros(N, SNAPSHOT_DTYPE.itemsize, dtype=t.uint8, device=self.device),
+                               t.from_numpy(self._partial.astype(np.uint8)).to(self.device),
+                               t.zeros(N, 6, dtype=t.float64, device=self.device))
+        return self._goal_bufs
+
+    def reset_goals_torch(self, rand_vec, env_mask=None, rand_vec_pass1=None):
+        """Restarts the envs with `env_mask` set (bool CUDA tensor [num_envs]; None = all) at the goals `rand_vec` (float64
+        CUDA tensor [num_envs, 6]: each env's `_last_rand_vec`, in the leading columns when its task's is shorter), as a
+        reset with an unfrozen rand_vec does: the reference's reset() with `rand_vec_pass1` (same layout; None = `rand_vec`)
+        in the first reset_model pass.  Works in every autoreset mode, without host synchronisation; returns the
+        observations as `reset_torch(mask)` does.  An env whose goal is not finite is left as it is and gets fault bit 64
+        (`engine.raise_on_faults()` raises ValueError)."""
+        t, N = self.torch, self.num_envs
+        if self._needs_reset:
+            raise RuntimeError("reset() must be called before reset_goals_torch()")
+        for name, x in (("rand_vec", rand_vec), ("rand_vec_pass1", rand_vec_pass1)):
+            if x is not None or name == "rand_vec":
+                if not (isinstance(x, t.Tensor) and x.dtype == t.float64 and x.device == self.device and tuple(x.shape) == (N, 6)):
+                    raise ValueError(f"reset_goals_torch needs {name} as a float64 tensor of shape ({N}, 6) on {self.device}")
+        mask = self._torch_mask(env_mask)
+        rows, partial, goal = self._goal_buffers()
+        rv = rand_vec.contiguous()
+        self.engine.build_goal_rows(mask, rv, None if rand_vec_pass1 is None else rand_vec_pass1.contiguous(), partial, rows)
+        if self._last_obs is not None and not self.post.active:      # the previous call was the numpy `reset` / `step`
+            self.d_obs.copy_(t.from_numpy(np.asarray(self._last_obs, dtype=np.float32)))
+        self.engine.reset_rows(mask, rows, self.d_obs)
+        f = rows.view(t.float32)                   # the envs k_reset_rows restarted: finite goal and observation
+        ok = mask & t.isfinite(f[:, _ROW_OBS:_ROW_OBS + 39]).all(1) & t.isfinite(f[:, _ROW_TARGET:_ROW_TARGET + 3]).all(1)
+        goal.copy_(t.where(ok[:, None], rv, goal))
+        return self._restarted(ok)
+
+    def reset_goals(self, rand_vec, env_mask=None, rand_vec_pass1=None):
+        """`reset_goals_torch` from numpy: `rand_vec` (and `rand_vec_pass1`) float64 [num_envs, 6], `env_mask` numpy bool
+        [num_envs] or None (all).  Shapes, dtypes, the mask and the finiteness of the masked rows are checked before
+        anything changes (ValueError).  Returns the observations as `reset(options={"reset_mask": ...})` does: the new
+        episodes' first observations in the masked rows, the last ones returned in the others."""
+        N = self.num_envs
+        mask = np.ones(N, dtype=bool) if env_mask is None else np.asarray(env_mask)
+        if mask.shape != (N,) or mask.dtype != np.bool_:
+            raise ValueError(f"env_mask must be a numpy bool array of shape ({N},), got {mask.dtype} {mask.shape}")
+        vecs = []
+        for name, x in (("rand_vec", rand_vec), ("rand_vec_pass1", rand_vec_pass1)):
+            if x is None and name == "rand_vec_pass1":
+                vecs.append(None)
+                continue
+            a = np.asarray(x)
+            if a.shape != (N, 6) or a.dtype != np.float64:
+                raise ValueError(f"reset_goals needs {name} as a float64 array of shape ({N}, 6), got {a.dtype} {a.shape}")
+            if not np.isfinite(a[mask]).all():
+                raise ValueError(f"reset_goals: {name} has non-finite entries in the rows of masked envs")
+            vecs.append(a)
+        if self._needs_reset:
+            raise RuntimeError("reset() must be called before reset_goals()")
+        t = self.torch
+        obs = self._last_obs.copy() if self._last_obs is not None else self._last_obs_device().cpu().numpy().astype(self.obs_dtype)
+        d = [None if a is None else t.from_numpy(np.ascontiguousarray(a)).to(self.device) for a in vecs]
+        out = self.reset_goals_torch(d[0], t.from_numpy(mask).to(self.device), d[1])
+        idx = np.nonzero(mask)[0]
+        self._ep_len[idx] = 0
+        self._sync_ended_to_host()
+        obs[idx] = out.cpu().numpy()[idx]
+        self._last_obs, self._d_last_obs = obs, None
+        return obs
+
+    def sample_goals(self, rng, env_mask=None):
+        """Goals for `reset_goals`: for every env with `env_mask` set (numpy bool [num_envs]; None = all), in env order,
+        the two draws of a reset with an unfrozen rand_vec (`benchmarks.draw_rand_vec`: each env's task's
+        _random_reset_space and rejection loop) from `rng`, a numpy Generator or RandomState.  Returns numpy float64
+        (rand_vec, rand_vec_pass1) [num_envs, 6]; other rows are zero."""
+        N = self.num_envs
+        mask = np.ones(N, dtype=bool) if env_mask is None else np.asarray(env_mask)
+        if mask.shape != (N,) or mask.dtype != np.bool_:
+            raise ValueError(f"env_mask must be a numpy bool array of shape ({N},), got {mask.dtype} {mask.shape}")
+        rv, rv1 = np.zeros((N, 6)), np.zeros((N, 6))
+        for e in np.nonzero(mask)[0]:
+            spec = TASKS[self.sub[e].task_name]
+            first = draw_rand_vec(spec, rng)
+            second = draw_rand_vec(spec, rng)
+            rv1[e, :first.size], rv[e, :second.size] = first, second
+        return rv, rv1
+
+    def _goal_task(self, e, v):
+        """The Task of env e's running episode on goal `v` (a reset_goals row)."""
+        name = self.sub[e].task_name
+        return make_task(name, np.array(v[:TASKS[name].rand_low.size], dtype=np.float64), bool(self._partial[e]))
 
     # ------------------------------------------------------------------ state accessors (SawyerXYZEnv / MujocoEnv getters)
     def query_torch(self, env_mask=None, bodies=(), sites=(), geoms=(), touching=False):
@@ -927,9 +1045,13 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
 
     # attribute RPC used by metaworld/evaluation.py:48-169 and the reference tests
     def _current_tasks(self):
-        if self._device_sampler:       # the device chose the goals: read the snapshot id of every env's running episode
+        if self._device_sampler or self._goal_bufs is not None:
+            # the device chose the goals (sampler), or an episode may run on a reset_goals goal (snapshot id -1): read the
+            # snapshot id of every env's running episode
             snap = self.engine.get_state()["snapshot"].astype(np.int64)
-            return [self._task_of_snap[int(i)] for i in snap]
+            goal = None if self._goal_bufs is None else self._goal_bufs[2].cpu().numpy()
+            return [self._goal_task(e, goal[e]) if i < 0 else self._task_of_snap[int(i)] if self._device_sampler
+                    else self.sub[e].current_task for e, i in enumerate(snap)]
         return [s.current_task for s in self.sub]
 
     def get_attr(self, name):
@@ -1009,6 +1131,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         record (qpos/qvel/warm start/mocap/frame stack/reward latches/episode counters) and the host mirrors, so a resumed
         run continues bit-identically mid-episode."""
         st = self.engine.get_state() if (physics and not self._needs_reset) else None
+        goal = None if st is None or self._goal_bufs is None else self._goal_bufs[2].cpu().numpy()
         out = []
         for e, s in enumerate(self.sub):
             tasks, idx, rng_state = s._pre if s._pre is not None else (s.tasks, s.current_task_idx, s.np_random.bit_generator.state)
@@ -1026,6 +1149,8 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
                    "current_task": None if s.current_task is None else _serialize_task(s.current_task)}
             if st is not None:
                 ext["state"] = base64.b64encode(st[e].tobytes()).decode("ascii")
+                if st[e]["snapshot"] < 0:        # an episode on a reset_goals goal
+                    ext["goal"] = [float(x) for x in goal[e]]
             ck["mw_b200"] = ext
             out.append((s.env_id, ck))
         return tuple(out)
@@ -1055,7 +1180,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             new_tasks += [_deserialize_task(t) for t in ck["tasks"]]
         self._ensure_snapshots(new_tasks)
         st = None
-        rows, lens, cur = [], [], []
+        rows, lens, cur, goals = [], [], [], {}
         for e, (s, ck) in enumerate(zip(self.sub, mine)):
             s.pending, s._pre = None, None
             s.tasks = [_deserialize_task(t) for t in ck["tasks"]]
@@ -1078,14 +1203,21 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
                     if st is None:
                         st = self.engine.get_state()
                     st[e] = np.frombuffer(base64.b64decode(ext["state"]), dtype=ENVSTATE_DTYPE)[0]
+                    if "goal" in ext:
+                        goals[e] = ext["goal"]
         # (the ended mark: a run stopped between a terminal step and its restart)
         self._restore_mirrors(rows, lens, cur, None if st is None else st["ended"][rows] != 0)
         if st is not None:
             # snapshot ids are engine-local: re-point every restored record at this engine's id for the same task
+            # (an episode on a reset_goals goal keeps snapshot id -1 and takes its running goal back)
             for e, s in enumerate(self.sub):
-                if s.current_task is not None:
+                if s.current_task is not None and e not in goals:
                     self._ensure_snapshots([s.current_task])
                     st[e]["snapshot"] = self._snap(s.current_task)
+            if goals:
+                g = self._goal_buffers()[2]
+                for e, v in goals.items():
+                    g[e] = self.torch.tensor(v, dtype=self.torch.float64)
             self.engine.set_state(st)
             self._needs_reset = False
         if not self._needs_reset:
