@@ -116,7 +116,40 @@ class _SubEnv:
             self.current_task = self.next_task()
 
 
-_ENDED_WORD = ENVSTATE_DTYPE.fields["ended"][1] // 4       # the ended mark's float32 word in a 512-byte state record
+class _Mirrored:
+    """One per-env value that the numpy calls read and write on the host (a numpy array) and the `_torch` calls on the
+    device (a tensor).  A write records the side it happened on and drops the other copy; a read of the other side
+    converts once (`to_host` / `to_device`) and keeps both copies until the next write."""
+
+    def __init__(self, to_host, to_device, host=None):
+        self._to_host, self._to_device = to_host, to_device
+        self._host, self._device = host, None
+
+    def set(self, host=None, device=None):
+        """The value was just written: on the host, on the device, or on both when the two are equal."""
+        self._host, self._device = host, device
+
+    def on_host(self):
+        return self._host is not None
+
+    def host(self, write=False):
+        """The host copy; `write`: the caller changes it in place, so the device copy is dropped."""
+        if self._host is None:
+            self._host = self._to_host(self._device)
+        if write:
+            self._device = None
+        return self._host
+
+    def device(self, write=False):
+        """The device copy; `write`: the caller changes it in place, so the host copy is dropped."""
+        if self._device is None:
+            self._device = self._to_device(self._host)
+        if write:
+            self._host = None
+        return self._device
+
+
+_ENDED_WORD = ENVSTATE_DTYPE.fields["ended"][1] // 4      # the ended mark's float32 word in a 512-byte state record
 # the float32 words of a 768-byte goal row (engine.build_goal_rows) that mw_reset_rows checks: _target_pos and the observation
 _ROW_TARGET = ENVSTATE_DTYPE.fields["target"][1] // 4
 _ROW_OBS = SNAPSHOT_DTYPE.fields["obs"][1] // 4
@@ -264,11 +297,12 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self._needs_reset = True
         self._device_sampler = False
         # NEXT_STEP / DISABLED: envs whose last step ended their episode and that have not restarted (the engine's `ended`
-        # flag).  The numpy path keeps it on the host, the torch path on the device; `_ended_on_device` says where it is now
-        self._ended = np.zeros(N, dtype=bool)
-        self.d_ended = torch.zeros(N, dtype=torch.bool, device=dev)
-        self._ended_on_device = False
-        self._last_obs = self._d_last_obs = None        # what the last call returned (unmasked rows of a partial reset)
+        # flag).  Its device copy is always this one buffer, which step_torch writes in place
+        d_marks = torch.zeros(N, dtype=torch.bool, device=dev)
+        self._autoreset_envs = _Mirrored(lambda d: d.cpu().numpy().copy(), lambda h: d_marks.copy_(torch.from_numpy(h)),
+                                         host=np.zeros(N, dtype=bool))
+        # what the last call returned (the unmasked rows of a partial reset)
+        self._returned_obs = _Mirrored(lambda d: d.cpu().numpy().astype(self.obs_dtype), self._obs_to_device)
         # optional per-sub-env wrappers of the reference that sit above the one-hot wrapper (metaworld/__init__.py:437-444);
         # one instance (one set of statistics) serves both `step` and `step_torch`
         from .post import StepPost
@@ -287,6 +321,48 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
     def _set_engine_options(self):
         # SawyerXYZEnv truncates at its own max_path_length = 500 whatever the TimeLimit wrapper says (sawyer_xyz_env.py:634)
         self.engine.set_options(min(self.max_episode_steps, MAX_PATH_LENGTH), self.terminate_on_success, self._seed)
+
+    def _obs_to_device(self, obs):
+        """A returned numpy observation as a float32 device tensor.  Without the optional wrappers that tensor is `d_obs`
+        itself, so a masked restart writes its rows straight into it."""
+        x = self.torch.from_numpy(np.asarray(obs, dtype=np.float32))
+        return x.to(self.device) if self.post.active else self.d_obs.copy_(x)
+
+    def _host_mask(self, env_mask, name="env_mask"):
+        """A numpy bool mask [num_envs], checked; None = every env."""
+        N = self.num_envs
+        m = np.ones(N, dtype=bool) if env_mask is None else np.asarray(env_mask)
+        if m.shape != (N,) or m.dtype != np.bool_:
+            raise ValueError(f"{name} must be a numpy bool array of shape ({N},), got {m.dtype} {m.shape}")
+        return m
+
+    def _device_mask(self, env_mask):
+        """A numpy bool mask [num_envs], checked and uploaded for a `_torch` call; None (every env) stays None."""
+        return None if env_mask is None else self.torch.from_numpy(self._host_mask(env_mask)).to(self.device)
+
+    def _check_tensor(self, name, x, dtype, shape, min_cols=None, contiguous=False):
+        """Raises ValueError unless `x` is a tensor on this env's device of `dtype` ("integer": any dtype that is not
+        floating point) and of `shape`; with `min_cols`, of shape [*shape, >= min_cols] with unit column stride (a column
+        slice of a wider tensor passes); with `contiguous`, contiguous."""
+        t = self.torch
+        ok = isinstance(x, t.Tensor) and x.device == self.device
+        ok = ok and (not x.is_floating_point() if dtype == "integer" else x.dtype == dtype)
+        if min_cols is None:
+            ok = ok and tuple(x.shape) == shape
+            want = str(shape)
+        else:
+            ok = ok and x.dim() == len(shape) + 1 and tuple(x.shape[:-1]) == shape and x.shape[-1] >= min_cols and x.stride(-1) == 1
+            want = f"({', '.join(map(str, shape))}, >= {min_cols})"
+        if not (ok and (not contiguous or x.is_contiguous())):
+            kind = "integer" if dtype == "integer" else str(dtype).removeprefix("torch.")
+            raise ValueError(f"{name} must be a {'contiguous ' if contiguous else ''}{kind} tensor of shape {want} on {self.device}")
+
+    def _torch_mask(self, env_mask, name="env_mask"):
+        """A bool device tensor [num_envs], checked and made contiguous; None = every env."""
+        if env_mask is None:
+            return self.d_all
+        self._check_tensor(name, env_mask, self.torch.bool, (self.num_envs,))
+        return env_mask.contiguous()
 
     @staticmethod
     def _task_key(slot, d):
@@ -362,11 +438,10 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         obs = self.h_obs.numpy().astype(self.obs_dtype)
         self._obs_template = obs.copy()        # constant columns (one-hot task id) of every later observation; see step()
         self._obs_template[:, :39] = 0
-        self._ended[:] = False
-        self._ended_on_device = False
+        self._autoreset_envs.set(host=np.zeros(self.num_envs, dtype=bool))
         if self.post.active:
             obs = self.post.on_reset(obs)
-        self._last_obs, self._d_last_obs = obs, None
+        self._returned_obs.set(host=obs, device=None if self.post.active else self.d_obs)   # (d_obs: the same values)
         return obs, {}
 
     def _reset_masked(self, mask):
@@ -382,9 +457,8 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         if self._device_sampler:
             raise RuntimeError("the device-side task sampler is active (step_torch was used): use reset_torch(reset_mask) or "
                                "disable_device_sampler() + reset()")
-        if self._last_obs is None:
+        if not self._returned_obs.on_host():
             raise RuntimeError("the last observations are on the device (step_torch): use reset_torch(reset_mask=...)")
-        self._sync_ended_to_host()
         idx = np.nonzero(mask)[0]
         self._take_reset_draws(idx)
         d_mask = self.torch.from_numpy(mask).to(self.device)
@@ -393,14 +467,14 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self.h_obs.copy_(self.d_obs)
         rows = self.h_obs.numpy()[idx].astype(self.obs_dtype)
         self._ep_len[idx] = 0
-        self._ended[idx] = False
-        obs = self._last_obs.copy()
+        self._autoreset_envs.host(write=True)[idx] = False
+        obs = self._returned_obs.host().copy()
         if self.post.active:
             full = np.zeros((N, rows.shape[1]), dtype=self.obs_dtype)
             full[idx] = rows
             rows = self.post.on_reset(full, mask)[idx]
         obs[idx] = rows
-        self._last_obs = obs
+        self._returned_obs.set(host=obs)
         return obs, {}
 
     def _merge_raw_rows(self, d_mask):
@@ -408,16 +482,6 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         the numpy `step`), the reset rows join them there."""
         if self._d_raw is self.d_obs39:
             self.d_obs39.copy_(self.torch.where(d_mask[:, None], self.d_obs[:, :39], self.d_obs39))
-
-    def _sync_ended_to_host(self):
-        if self._ended_on_device:
-            self._ended = self.d_ended.cpu().numpy().copy()
-            self._ended_on_device = False
-
-    def _sync_ended_to_device(self):
-        if not self._ended_on_device:
-            self.d_ended.copy_(self.torch.from_numpy(self._ended))
-            self._ended_on_device = True
 
     def _advance_streams(self, idx):
         """The autoreset's task-select draw of sub-envs `idx` (their episode ends with this step): the speculative draw
@@ -480,7 +544,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
             self._ep_len[idx] = 0
             if len(pred) < len(idx):                 # terminations nobody could predict (terminate_on_success)
                 self._advance_streams(np.setdiff1d(idx, pred))
-        self._last_obs = obs
+        self._returned_obs.set(host=obs)
         return obs, reward, terminated, truncated, infos
 
     def _step_deferred(self, actions):
@@ -490,11 +554,11 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         reward 0, no flags and no infos; their task-select draw becomes the running task then.  DISABLED: stepping an env
         that ended and was not reset (`reset(options={"reset_mask": ...})`) fails before anything is launched."""
         N = self.num_envs
-        self._sync_ended_to_host()
+        ended = self._autoreset_envs.host()
         if self.autoreset_mode == "Disabled":
-            assert not self._ended.any(), f"self._autoreset_envs={self._ended!r}"      # SyncVectorEnv's DISABLED assertion
-        restart = np.nonzero(self._ended)[0]      # (none under DISABLED)
-        a, pred = self._launch(actions)
+            assert not ended.any(), f"self._autoreset_envs={ended!r}"      # SyncVectorEnv's DISABLED assertion
+        restart = np.nonzero(ended)[0]      # (none under DISABLED)
+        a, pred = self._launch(actions, ended)
         if len(restart):                 # queued behind the kernel, which has read these envs' snapshot ids
             self._advance_streams(restart)
         obs, sm, reward, terminated, truncated = self._collect()
@@ -512,14 +576,15 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
                 ep_r = np.zeros(N)
                 ep_r[idx] = self._terminal_rows(idx, pred, self.h_final_info[:, 7], self.d_final_info[:, 7])
             infos["episode"], infos["_episode"] = self._episode_stats(done, ep_r)
-        self._ended = done
-        self._last_obs = obs
+        self._autoreset_envs.set(host=done)
+        self._returned_obs.set(host=obs)
         return obs, reward, terminated, truncated, infos
 
-    def _launch(self, actions):
+    def _launch(self, actions, ended=None):
         """Uploads `actions`, launches k_step and queues the copies of its results behind it: the packed [N, 9] record,
         the 39 observation columns it writes, and the terminal rows of the envs whose episode it truncates.  Those are known
         in advance (the host mirrors the episode lengths), so on most steps one synchronise brings back everything.
+        `ended` (NEXT_STEP / DISABLED): the envs that ended in the previous call, which restart or stand still.
         -> (the actions as a float32 [N, 4] array, the indices of those envs)"""
         t = self.torch
         a = np.ascontiguousarray(actions, dtype=np.float32).reshape(self.num_envs, 4)
@@ -530,8 +595,8 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         self._d_raw = self.d_obs39
         self.h_small.copy_(self.d_small, non_blocking=True)
         self.h_obs39.copy_(self.d_obs39, non_blocking=True)
-        # an env that ended in the previous call (NEXT_STEP / DISABLED; none under SAME_STEP) restarts or stands still
-        pred = np.nonzero((self._ep_len + 1 >= min(self.max_episode_steps, MAX_PATH_LENGTH)) & ~self._ended)[0]
+        due = self._ep_len + 1 >= min(self.max_episode_steps, MAX_PATH_LENGTH)
+        pred = np.nonzero(due if ended is None else due & ~ended)[0]
         npred = len(pred)
         if npred:
             self.h_idx[:npred] = t.from_numpy(pred)
@@ -612,45 +677,28 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
     def reset_torch(self, reset_mask=None):
         """Without a mask: `reset()`, result on the device.  `reset_mask` (bool CUDA tensor [num_envs]): only those envs
         restart, as `reset(options={"reset_mask": ...})` does, without host synchronisation: their snapshot comes from the
-        device sampler (or the pre-drawn task when no env re-samples), and the other rows are what the last
-        `step_torch` / `reset_torch` returned.  The returned tensor is overwritten by the next call."""
-        t = self.torch
+        device sampler (or the pre-drawn task when no env re-samples), and the other rows are what the previous call
+        returned.  The returned tensor is overwritten by the next call."""
         if reset_mask is None:
-            obs, _ = self.reset()
-            if not self.post.active:
-                out = self.d_obs
-            else:        # the wrapped observation of reset(): the wrappers' statistics see the reset observation once
-                out = t.from_numpy(np.asarray(obs, dtype=np.float32)).to(self.device)
-            self._d_last_obs = out
-            return out
+            self.reset()      # with the optional wrappers: their reset() output, so their statistics see it only once
+            return self._returned_obs.device()
         if self._needs_reset:
             raise RuntimeError("reset_torch() without a mask must come first")
-        if not (isinstance(reset_mask, t.Tensor) and reset_mask.dtype == t.bool and reset_mask.device == self.device
-                and tuple(reset_mask.shape) == (self.num_envs,)):
-            raise ValueError(f"reset_mask must be a bool tensor of shape ({self.num_envs},) on {self.device}")
+        mask = self._torch_mask(reset_mask, "reset_mask")
         if not self._device_sampler and any(s.sample_tasks_on_reset for s in self.sub):
             self.enable_device_sampler()
-        mask = reset_mask.contiguous()
-        if self._last_obs is not None and not self.post.active:      # the previous call was the numpy `reset` / `step`
-            self.d_obs.copy_(t.from_numpy(np.asarray(self._last_obs, dtype=np.float32)))
+        last = self._returned_obs.device()
         self.engine.reset_masked(mask, self.d_obs, None if self._device_sampler else self.d_next)
-        return self._restarted(mask)
+        return self._restarted(mask, last)
 
-    def _restarted(self, mask):
-        """The bookkeeping of a masked restart into `d_obs` (bool device tensor `mask`): base rows, ended marks, the
-        optional wrappers' reset; returns the observations as `reset_torch(mask)` does."""
-        t = self.torch
+    def _restarted(self, mask, last):
+        """The bookkeeping of a masked restart into `d_obs` (bool device tensor `mask`) from the observations `last` the
+        previous call returned, on the device (taken before the restart: without the optional wrappers they are `d_obs`):
+        base rows, ended marks, the optional wrappers' reset; returns the observations as `reset_torch(mask)` does."""
         self._merge_raw_rows(mask)
-        self._sync_ended_to_device()
-        self.d_ended &= ~mask
-        if not self.post.active:
-            out = self.d_obs
-        else:
-            last = self._d_last_obs
-            if last is None:         # the previous call was the numpy `reset` / `step`
-                last = t.from_numpy(np.asarray(self._last_obs, dtype=np.float32)).to(self.device)
-            out = t.where(mask[:, None], self.post.on_reset(self.d_obs, mask), last)
-        self._last_obs, self._d_last_obs = None, out
+        self._autoreset_envs.device(write=True).logical_and_(~mask)
+        out = self.torch.where(mask[:, None], self.post.on_reset(self.d_obs, mask), last) if self.post.active else last
+        self._returned_obs.set(device=out)
         return out
 
     def step_torch(self, actions):
@@ -659,53 +707,32 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         t = self.torch
         if self._needs_reset:
             raise RuntimeError("reset() must be called before step_torch()")
-        if not (isinstance(actions, t.Tensor) and actions.dtype == t.float32 and actions.device == self.device
-                and tuple(actions.shape) == (self.num_envs, 4) and actions.is_contiguous()):
-            raise ValueError(f"step_torch needs a contiguous float32 tensor of shape ({self.num_envs}, 4) on {self.device}")
+        self._check_tensor("actions", actions, t.float32, (self.num_envs, 4), contiguous=True)
         if not self._device_sampler and any(s.sample_tasks_on_reset for s in self.sub):
             self.enable_device_sampler()      # without it every autoreset would restart the same pre-drawn goal
         nxt = None if self._device_sampler else self.d_next
-        restart = None
+        ended = restart = None
         if self.autoreset_mode != "SameStep":      # NEXT_STEP restarts the envs that ended in the previous call
-            self._sync_ended_to_device()
-            restart = self.d_ended.clone() if self.autoreset_mode == "NextStep" else None
+            ended = self._autoreset_envs.device(write=True)
+            restart = ended.clone() if self.autoreset_mode == "NextStep" else None
         self.engine.step(actions, self.d_obs, self.d_reward, self.d_term, self.d_trunc, self.d_small, self.d_final_obs,
                          self.d_final_info, nxt)
         self._d_raw = self.d_obs
-        self._last_obs = None
-        if restart is not None or self.autoreset_mode == "Disabled":
-            t.logical_or(self.d_term, self.d_trunc, out=self.d_ended)
+        if ended is not None:
+            t.logical_or(self.d_term, self.d_trunc, out=ended)
+        obs, rew = self.d_obs, self.d_reward
         if self.post.active:       # the optional wrappers on the device; the terminal observation and episode returns stay available
             obs, rew, self.d_final_obs_post, self.d_episode_return_post = self.post.on_step(
                 self.d_obs, actions, self.d_reward, self.d_term, self.d_trunc,
                 self.d_final_obs if self.autoreset_mode == "SameStep" else None, restart=restart)
-            self._d_last_obs = obs
-            return obs, rew, self.d_term, self.d_trunc, self.d_info
-        return self.d_obs, self.d_reward, self.d_term, self.d_trunc, self.d_info
+        self._returned_obs.set(device=obs)
+        return obs, rew, self.d_term, self.d_trunc, self.d_info
 
     # ------------------------------------------------------------------ physics state (MujocoEnv.set_state, get_env_state, _get_obs)
     # The optional wrappers are not involved: the reference's `call` reaches these methods on the base env.
     def _check_started(self, what):
         if self._needs_reset:
             raise RuntimeError(f"reset() must be called before {what} (the device state is created by reset)")
-
-    def _device_mask(self, env_mask):
-        """numpy bool [num_envs] or None (every env) -> the device tensor."""
-        if env_mask is None:
-            return self.d_all
-        m = np.asarray(env_mask)
-        if m.shape != (self.num_envs,) or m.dtype != np.bool_:
-            raise ValueError(f"env_mask must be a numpy bool array of shape ({self.num_envs},), got {m.dtype} {m.shape}")
-        return self.torch.from_numpy(m).to(self.device)
-
-    def _torch_mask(self, env_mask):
-        t = self.torch
-        if env_mask is None:
-            return self.d_all
-        if not (isinstance(env_mask, t.Tensor) and env_mask.dtype == t.bool and env_mask.device == self.device
-                and tuple(env_mask.shape) == (self.num_envs,)):
-            raise ValueError(f"env_mask must be a bool tensor of shape ({self.num_envs},) on {self.device}")
-        return env_mask.contiguous()
 
     def set_state(self, qpos, qvel, env_mask=None):
         """MujocoEnv.set_state for the envs with `env_mask` set (numpy bool [num_envs]; None = all): `qpos` [num_envs, 18]
@@ -717,27 +744,23 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         qpos, qvel = np.asarray(qpos, dtype=np.float64), np.asarray(qvel, dtype=np.float64)
         if qpos.shape != (N, MAXNQ) or qvel.shape != (N, MAXDOF):
             raise ValueError(f"set_state needs qpos of shape ({N}, {MAXNQ}) and qvel of shape ({N}, {MAXDOF}), got {qpos.shape} and {qvel.shape}")
-        mask = self._device_mask(env_mask)
-        rows = np.ones(N, dtype=bool) if env_mask is None else np.asarray(env_mask)
+        rows = self._host_mask(env_mask)
         nq, nv = self._getters.dims()
         used_q = (np.arange(MAXNQ) < nq[:, None]) & rows[:, None]
         used_v = (np.arange(MAXDOF) < nv[:, None]) & rows[:, None]
         if not (np.isfinite(qpos[used_q]).all() and np.isfinite(qvel[used_v]).all()):
             raise ValueError("set_state: qpos / qvel of the selected envs must be finite")
         t = self.torch
-        self.engine.set_physics(mask, t.from_numpy(np.ascontiguousarray(qpos)).to(self.device),
-                                t.from_numpy(np.ascontiguousarray(qvel)).to(self.device))
+        self.set_state_torch(t.from_numpy(np.ascontiguousarray(qpos)).to(self.device),
+                             t.from_numpy(np.ascontiguousarray(qvel)).to(self.device), self._device_mask(env_mask))
 
     def set_state_torch(self, qpos, qvel, env_mask=None):
         """`set_state` from device tensors, without host synchronisation: `qpos` float64 [num_envs, 18], `qvel` float64
         [num_envs, 17], contiguous, on this env's device; `env_mask` a bool tensor [num_envs] or None (all).  Values are not
         inspected (a non-finite state shows up as a non-finite observation fault)."""
         self._check_started("set_state_torch")
-        t = self.torch
-        for name, x, w in (("qpos", qpos, MAXNQ), ("qvel", qvel, MAXDOF)):
-            if not (isinstance(x, t.Tensor) and x.dtype == t.float64 and x.device == self.device
-                    and tuple(x.shape) == (self.num_envs, w) and x.is_contiguous()):
-                raise ValueError(f"set_state_torch needs {name} as a contiguous float64 tensor of shape ({self.num_envs}, {w}) on {self.device}")
+        self._check_tensor("qpos", qpos, self.torch.float64, (self.num_envs, MAXNQ), contiguous=True)
+        self._check_tensor("qvel", qvel, self.torch.float64, (self.num_envs, MAXDOF), contiguous=True)
         self.engine.set_physics(self._torch_mask(env_mask), qpos, qvel)
 
     def get_state_torch(self):
@@ -763,8 +786,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
     def observe(self, env_mask=None):
         """`observe_torch` with a numpy bool mask (None = all); a float64 numpy array [num_envs, obs_dim]."""
         self._check_started("observe")
-        self.engine.observe(self._device_mask(env_mask), self.d_env_obs)
-        return self.d_env_obs.cpu().numpy().astype(np.float64)
+        return self.observe_torch(self._device_mask(env_mask)).cpu().numpy().astype(np.float64)
 
     # ------------------------------------------------------------------ saved states (save, restore and fork on the device)
     # A loaded env continues bit for bit as its source would have, up to the end of the current episode, in every autoreset
@@ -778,15 +800,13 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         all), without host synchronisation (with a numpy mask: one upload)."""
         self._check_started("save_states")
         t, N = self.torch, self.num_envs
-        mask = self._torch_mask(env_mask) if isinstance(env_mask, t.Tensor) else self._device_mask(env_mask)
+        if env_mask is not None:
+            env_mask = self._torch_mask(env_mask) if isinstance(env_mask, t.Tensor) else self._device_mask(env_mask)
         records = t.zeros(N, 512, dtype=t.uint8, device=self.device)
         model = t.full((N,), -1, dtype=t.int32, device=self.device)
         hints = t.zeros(N, NCONV, 4, dtype=t.float32, device=self.device)
-        self.engine.save_states(records, model, hints, None if env_mask is None else mask)
-        if self._last_obs is not None:
-            obs = self._last_obs.copy()
-        else:
-            obs = (self._d_last_obs if self.post.active else self.d_obs).clone()
+        self.engine.save_states(records, model, hints, env_mask)
+        obs = self._returned_obs.host().copy() if self._returned_obs.on_host() else self._returned_obs.device().clone()
         return EnvStates(self, records, model, hints, self._d_raw[:, :39].clone(), obs,
                          self.post.save_rows() if self.post.active else None, self._ep_len.copy(),
                          [s.current_task for s in self.sub], None if self._goal_bufs is None else self._goal_bufs[2].clone())
@@ -796,15 +816,11 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         if not isinstance(states, EnvStates) or states.owner is not self:
             raise ValueError(f"{what}: the states were saved by another env (snapshot ids are engine-local)")
 
-    def _restore_mirrors(self, rows, ep_len, tasks, ended):
-        """The host mirrors of envs `rows` as a saved state has them: episode lengths, running tasks and (unless `ended` is
-        None) ended marks."""
+    def _restore_mirrors(self, rows, ep_len, tasks):
+        """The host mirrors of envs `rows` as a saved state has them: episode lengths and running tasks."""
         self._ep_len[rows] = ep_len
         for e, tk in zip(rows, tasks):
             self.sub[e].current_task = tk
-        if ended is not None:
-            self._sync_ended_to_host()
-            self._ended[rows] = ended
 
     def load_states(self, states, env_mask=None, src=None):
         """Env e with `env_mask[e]` set (numpy bool [num_envs]; None = all) takes row `src[e]` (numpy integers [num_envs];
@@ -814,9 +830,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         reset continue with the loaded task after the episode; the others keep their own task streams."""
         self._check_states(states, "load_states")
         N = self.num_envs
-        mask = np.ones(N, dtype=bool) if env_mask is None else np.asarray(env_mask)
-        if mask.shape != (N,) or mask.dtype != np.bool_:
-            raise ValueError(f"env_mask must be a numpy bool array of shape ({N},), got {mask.dtype} {mask.shape}")
+        mask = self._host_mask(env_mask)
         src = np.arange(N) if src is None else np.asarray(src)
         if src.shape != (N,) or src.dtype.kind not in "iu":
             raise ValueError(f"src must be a numpy integer array of shape ({N},)")
@@ -829,29 +843,14 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         if len(bad):
             raise ValueError(f"load_states: env(s) {bad.tolist()[:8]} have no saved state of their model at the given src")
         t = self.torch
-        d_mask = t.from_numpy(mask).to(self.device)
-        d_src = t.from_numpy(src.astype(np.int32)).to(self.device)
-        self.engine.load_states(states.records, states.model, states.hints, d_mask, d_src)
-        self._restore_mirrors(rows, states.ep_len[s], [states.tasks[i] for i in s], states.ended().cpu().numpy()[s])
+        self.load_states_torch(states, t.from_numpy(mask).to(self.device), t.from_numpy(src.astype(np.int32)).to(self.device))
+        self._restore_mirrors(rows, states.ep_len[s], [states.tasks[i] for i in s])
         for e in rows:
             if not self.sub[e].sample_tasks_on_reset:
                 self._draw_pending(e)
         self._push_next()
-        self._d_raw[:, :39] = t.where(d_mask[:, None], states.raw[d_src.long()], self._d_raw[:, :39])
-        self._load_goals(states, d_mask, d_src.long())
-        saved = states.obs if isinstance(states.obs, np.ndarray) else states.obs.cpu().numpy()
-        obs = (self._last_obs if self._last_obs is not None else self._last_obs_device().cpu().numpy()).astype(self.obs_dtype)
-        obs[rows] = saved[s]
-        if self.post.active:
-            self.post.load_rows(states.post, mask, src)
-        self._last_obs = obs
-        return obs
-
-    def _last_obs_device(self):
-        """What the last call returned, as a device tensor."""
-        if self._last_obs is not None:
-            return self.torch.from_numpy(np.asarray(self._last_obs, dtype=np.float32)).to(self.device)
-        return self._d_last_obs if self.post.active else self.d_obs
+        self._autoreset_envs.host()        # fetched here, not by the next numpy `step`
+        return self._returned_obs.host()
 
     def load_states_torch(self, states, env_mask=None, src=None):
         """`load_states` from device tensors, without host synchronisation: `env_mask` a bool tensor [num_envs] or None (all),
@@ -864,29 +863,27 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         mask = self._torch_mask(env_mask)
         if src is None:
             src = t.arange(N, device=self.device)
-        elif not (isinstance(src, t.Tensor) and src.device == self.device and not src.is_floating_point()
-                  and tuple(src.shape) == (N,)):
-            raise ValueError(f"src must be an integer tensor of shape ({N},) on {self.device}")
+        else:
+            self._check_tensor("src", src, "integer", (N,))
         src = src.long()
         sc = src.clamp(0, N - 1)
         ok = mask & (src >= 0) & (src < N) & (states.model[sc] == self.d_env_model)    # the check of k_load_states
         self.engine.load_states(states.records, states.model, states.hints, None if env_mask is None else mask,
                                 src.to(t.int32))
         if self.autoreset_mode != "SameStep":
-            self._sync_ended_to_device()
-            self.d_ended.copy_(t.where(ok, states.ended()[sc], self.d_ended))
+            ended = self._autoreset_envs.device(write=True)
+            ended.copy_(t.where(ok, states.ended()[sc], ended))
         self._d_raw[:, :39] = t.where(ok[:, None], states.raw[sc], self._d_raw[:, :39])
         self._load_goals(states, ok, sc)
         saved = states.obs
         if isinstance(saved, np.ndarray):          # saved right after a numpy call
             saved = t.from_numpy(saved.astype(np.float32)).to(self.device)
-        out = t.where(ok[:, None], saved[sc], self._last_obs_device())
+        out = t.where(ok[:, None], saved[sc], self._returned_obs.device())
         if self.post.active:
             self.post.load_rows(states.post, ok, sc)
         else:
-            self.d_obs.copy_(out)
-            out = self.d_obs
-        self._last_obs, self._d_last_obs = None, out
+            out = self.d_obs.copy_(out)
+        self._returned_obs.set(device=out)
         return out
 
     def _load_goals(self, states, mask, src):
@@ -920,21 +917,19 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         t, N = self.torch, self.num_envs
         if self._needs_reset:
             raise RuntimeError("reset() must be called before reset_goals_torch()")
-        for name, x in (("rand_vec", rand_vec), ("rand_vec_pass1", rand_vec_pass1)):
-            if x is not None or name == "rand_vec":
-                if not (isinstance(x, t.Tensor) and x.dtype == t.float64 and x.device == self.device and tuple(x.shape) == (N, 6)):
-                    raise ValueError(f"reset_goals_torch needs {name} as a float64 tensor of shape ({N}, 6) on {self.device}")
+        self._check_tensor("rand_vec", rand_vec, t.float64, (N, 6))
+        if rand_vec_pass1 is not None:
+            self._check_tensor("rand_vec_pass1", rand_vec_pass1, t.float64, (N, 6))
         mask = self._torch_mask(env_mask)
         rows, partial, goal = self._goal_buffers()
         rv = rand_vec.contiguous()
         self.engine.build_goal_rows(mask, rv, None if rand_vec_pass1 is None else rand_vec_pass1.contiguous(), partial, rows)
-        if self._last_obs is not None and not self.post.active:      # the previous call was the numpy `reset` / `step`
-            self.d_obs.copy_(t.from_numpy(np.asarray(self._last_obs, dtype=np.float32)))
+        last = self._returned_obs.device()
         self.engine.reset_rows(mask, rows, self.d_obs)
         f = rows.view(t.float32)                   # the envs k_reset_rows restarted: finite goal and observation
         ok = mask & t.isfinite(f[:, _ROW_OBS:_ROW_OBS + 39]).all(1) & t.isfinite(f[:, _ROW_TARGET:_ROW_TARGET + 3]).all(1)
         goal.copy_(t.where(ok[:, None], rv, goal))
-        return self._restarted(ok)
+        return self._restarted(ok, last)
 
     def reset_goals(self, rand_vec, env_mask=None, rand_vec_pass1=None):
         """`reset_goals_torch` from numpy: `rand_vec` (and `rand_vec_pass1`) float64 [num_envs, 6], `env_mask` numpy bool
@@ -942,9 +937,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         anything changes (ValueError).  Returns the observations as `reset(options={"reset_mask": ...})` does: the new
         episodes' first observations in the masked rows, the last ones returned in the others."""
         N = self.num_envs
-        mask = np.ones(N, dtype=bool) if env_mask is None else np.asarray(env_mask)
-        if mask.shape != (N,) or mask.dtype != np.bool_:
-            raise ValueError(f"env_mask must be a numpy bool array of shape ({N},), got {mask.dtype} {mask.shape}")
+        mask = self._host_mask(env_mask)
         vecs = []
         for name, x in (("rand_vec", rand_vec), ("rand_vec_pass1", rand_vec_pass1)):
             if x is None and name == "rand_vec_pass1":
@@ -959,14 +952,14 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         if self._needs_reset:
             raise RuntimeError("reset() must be called before reset_goals()")
         t = self.torch
-        obs = self._last_obs.copy() if self._last_obs is not None else self._last_obs_device().cpu().numpy().astype(self.obs_dtype)
+        obs = self._returned_obs.host().copy()
         d = [None if a is None else t.from_numpy(np.ascontiguousarray(a)).to(self.device) for a in vecs]
         out = self.reset_goals_torch(d[0], t.from_numpy(mask).to(self.device), d[1])
         idx = np.nonzero(mask)[0]
         self._ep_len[idx] = 0
-        self._sync_ended_to_host()
+        self._autoreset_envs.host()        # fetched here, not by the next numpy `step`
         obs[idx] = out.cpu().numpy()[idx]
-        self._last_obs, self._d_last_obs = obs, None
+        self._returned_obs.set(host=obs)
         return obs
 
     def sample_goals(self, rng, env_mask=None):
@@ -975,9 +968,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         _random_reset_space and rejection loop) from `rng`, a numpy Generator or RandomState.  Returns numpy float64
         (rand_vec, rand_vec_pass1) [num_envs, 6]; other rows are zero."""
         N = self.num_envs
-        mask = np.ones(N, dtype=bool) if env_mask is None else np.asarray(env_mask)
-        if mask.shape != (N,) or mask.dtype != np.bool_:
-            raise ValueError(f"env_mask must be a numpy bool array of shape ({N},), got {mask.dtype} {mask.shape}")
+        mask = self._host_mask(env_mask)
         rv, rv1 = np.zeros((N, 6)), np.zeros((N, 6))
         for e in np.nonzero(mask)[0]:
             spec = TASKS[self.sub[e].task_name]
@@ -1024,10 +1015,8 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         if obs is None:
             self._check_started("expert_actions_torch")
             obs = self._d_raw
-        elif not (isinstance(obs, t.Tensor) and obs.dtype == t.float32 and obs.device == self.device and obs.dim() == 2
-                  and obs.shape[0] == self.num_envs and obs.shape[1] >= 39 and obs.stride(1) == 1):
-            raise ValueError(f"expert_actions_torch needs obs as a float32 tensor of shape ({self.num_envs}, >= 39) with "
-                             f"contiguous rows on {self.device}")
+        else:
+            self._check_tensor("obs", obs, t.float32, (self.num_envs,), min_cols=39)
         if self._d_expert_ids is None:
             self._d_expert_ids = t.tensor([TASK_IDS.get(s.task_name, -1) for s in self.sub], dtype=t.int32, device=self.device)
         out = t.empty(self.num_envs, 4, dtype=t.float32, device=self.device)
@@ -1205,9 +1194,10 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
                     st[e] = np.frombuffer(base64.b64decode(ext["state"]), dtype=ENVSTATE_DTYPE)[0]
                     if "goal" in ext:
                         goals[e] = ext["goal"]
-        # (the ended mark: a run stopped between a terminal step and its restart)
-        self._restore_mirrors(rows, lens, cur, None if st is None else st["ended"][rows] != 0)
+        self._restore_mirrors(rows, lens, cur)
         if st is not None:
+            # (the ended mark: a run stopped between a terminal step and its restart)
+            self._autoreset_envs.host(write=True)[rows] = st["ended"][rows] != 0
             # snapshot ids are engine-local: re-point every restored record at this engine's id for the same task
             # (an episode on a reset_goals goal keeps snapshot id -1 and takes its running goal back)
             for e, s in enumerate(self.sub):

@@ -42,7 +42,7 @@ def _run(v, acts):
     return [v.step(a) for a in acts]
 
 
-def test_load_restores_host_mirrors_wrapper_rows_and_replays():
+def test_load_restores_ended_marks_mirrors_wrapper_rows_and_replays():
     """MT10 x 3 replicas on the oracle, NEXT_STEP, every optional wrapper.  A masked reset staggers the episodes, so at the
     save some envs have just ended and the others are mid-episode.  Loading with `src` permuted among the envs of each
     type gives every env its source's episode length, ended mark, running task, wrapper rows and last observation;
@@ -61,7 +61,7 @@ def test_load_restores_host_mirrors_wrapper_rows_and_replays():
     last = _run(v, acts[3:9])[-1][0]
     v.call("toggle_sample_tasks_on_reset", False)         # a restart then draws the same task in both runs
     st = v.save_states()
-    ep_len, ended = v._ep_len.copy(), v._ended.copy()
+    ep_len, ended = v._ep_len.copy(), v._autoreset_envs.host().copy()
     assert ended.any() and not ended.all() and len(set(ep_len)) > 1
     rv = v.get_attr("_last_rand_vec")
     post = v.post.save_rows()
@@ -70,7 +70,7 @@ def test_load_restores_host_mirrors_wrapper_rows_and_replays():
     # permuted within each env type (env e has type e % 10)
     src = np.arange(N).reshape(3, 10)[[1, 2, 0]].reshape(-1)
     obs = v.load_states(st, src=src)
-    assert np.array_equal(v._ep_len, ep_len[src]) and np.array_equal(v._ended, ended[src])
+    assert np.array_equal(v._ep_len, ep_len[src]) and np.array_equal(v._autoreset_envs.host(), ended[src])
     assert all(np.array_equal(x, rv[s]) for x, s in zip(v.get_attr("_last_rand_vec"), src))
     rows = v.post.save_rows()
     assert rows.keys() == post.keys() and all(np.array_equal(rows[k], post[k][src]) for k in post)

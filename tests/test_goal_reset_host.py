@@ -94,7 +94,7 @@ def _same(a, b):
     return np.array_equal(a, b)
 
 
-def test_reset_goals_host_logic():
+def test_reset_goals_checks_inputs_and_equals_a_masked_reset_from_snapshots():
     """MT10 x 2 replicas on the oracle with observation normalisation.  `reset_goals` checks its inputs before anything
     changes.  It is, by definition, `engine.reset_masked` from snapshots built for the same goals (twin `u`): same
     observations, wrapper rows and next steps.  It zeroes the episode lengths and ended marks of the masked envs only,
@@ -127,12 +127,13 @@ def test_reset_goals_host_logic():
     ids = np.zeros(N, dtype=np.int32)
     ids[rows] = u.engine.build_snapshots(u._env_model[rows], rv[rows], u._partial[rows], rand_vec_pass1=rv1[rows])
     d_mask = torch.from_numpy(mask)
+    last = u._returned_obs.device()
     u.engine.reset_masked(d_mask, u.d_obs, torch.from_numpy(ids))
-    want = u._last_obs.copy()
-    want[rows] = u._restarted(d_mask).numpy()[rows]
-    u._last_obs = want
+    want = u._returned_obs.host().copy()
+    want[rows] = u._restarted(d_mask, last).numpy()[rows]
+    u._returned_obs.set(host=want)
     assert obs.dtype == want.dtype and np.array_equal(obs, want)
-    assert np.array_equal(v._ep_len, np.where(mask, 0, 3)) and not v._ended.any()
+    assert np.array_equal(v._ep_len, np.where(mask, 0, 3)) and not v._autoreset_envs.host().any()
     assert np.array_equal(v.engine.get_state()["snapshot"][rows], -np.ones(len(rows)))
     n = [len(x) for x in w.get_attr("_last_rand_vec")]
     got, old = v.get_attr("_last_rand_vec"), w.get_attr("_last_rand_vec")

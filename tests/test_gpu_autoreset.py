@@ -172,7 +172,7 @@ def test_step_and_step_torch_agree_exactly_under_next_step_with_wrappers(torch_c
     a.close(); b.close()
 
 
-def test_next_step_checkpoint_between_terminal_step_and_restart_resumes_bitwise(torch_cuda):
+def test_next_step_checkpoint_taken_before_the_restart_resumes_bitwise(torch_cuda):
     from metaworld_b200.vector_env import make_mt_envs
     kw = dict(seed=11, num_envs=20, max_episode_steps=5, use_one_hot=True, terminate_on_success=True, autoreset_mode="NextStep")
     rng = np.random.default_rng(0)
@@ -181,7 +181,7 @@ def test_next_step_checkpoint_between_terminal_step_and_restart_resumes_bitwise(
     a.reset()
     for t in range(5):
         a.step(A[t])                 # the 5th step truncates every env that did not succeed earlier
-    assert a._ended.any()
+    assert a._autoreset_envs.host().any()
     ck = a.call("get_checkpoint")
     ref = [a.step(A[t]) for t in range(5, 30)]
     b = make_mt_envs("MT10", **kw)
