@@ -11,16 +11,31 @@ TEST INFRASTRUCTURE: each call mirrors what its kernel (csrc/mw_engine.cu) does 
 * `query` mirrors `k_query`: a forward pass of the current state, then the observation frame without committing the
   frame stack, the named poses (NaN for a missing name) and touching_object of the slot's geom.  Sites a task's
   reset_model places through model.site(name).pos are posed as the kernel poses them (their body + _target_pos /
-  obj_init_pos): the oracle leaves some of them at the model file's place."""
+  obj_init_pos): the oracle leaves some of them at the model file's place;
+* `build_goal_rows` / `reset_rows` mirror `k_goal_rows` / `k_reset_rows`.  A goal row is what rebuilds the episode
+  start: (model slot, rand_vec, observability, rand_vec_pass1).  Of the 768 bytes the host reads only the words
+  k_reset_rows checks, the observation and _target_pos, to know which envs restarted; the stand-in writes them finite
+  for a finite goal and NaN otherwise, as the kernel's rows are.  `reset_rows` restarts the env from the row's goal by
+  the oracle's reset() with the two passes' vectors, records snapshot id -1 and skips a row with a non-finite goal, as
+  k_reset_rows leaves such an env unchanged;
+* `save_states` / `load_states` mirror `k_save_states` / `k_load_states`.  An oracle env's state lives in C memory that
+  cannot be copied, so a saved row is what rebuilds it: the definition of the episode's start (a snapshot's or a goal
+  row's), the calls that changed the env since (steps, set_physics, observe) and the counters.  Loading restarts the
+  target env from that definition and replays the calls, so the target continues exactly as the source would.  The
+  record rows get the state record (the host reads the ended mark there) and the model slot; a row out of range or of
+  another model is skipped, as k_load_states leaves such an env unchanged."""
 import numpy as np
 import torch
 from scipy.spatial.transform import Rotation
 
 from metaworld_b200 import modelzoo
-from metaworld_b200.engine import ENVSTATE_DTYPE, INFO_KEYS
+from metaworld_b200.engine import ENVSTATE_DTYPE, INFO_KEYS, SNAPSHOT_DTYPE
 from metaworld_b200.tasks import MOVED_SITES, TASKS
 from oracle import mjphys as P
 from oracle.tasks import TASKS as OT
+
+_OBS = SNAPSHOT_DTYPE.fields["obs"][1] // 4
+_TARGET = ENVSTATE_DTYPE.fields["target"][1] // 4
 
 
 class OracleEngine:
@@ -28,7 +43,7 @@ class OracleEngine:
         self.torch = torch
         self.device = torch.device("cpu")
         self.names = list(names)
-        self.snaps = []           # (slot, rand_vec, partially_observable)
+        self.snaps = []           # episode starts: (slot, rand_vec, partially_observable, rand_vec_pass1)
         self.max_steps, self.tos = 500, False
         self.mode = "SameStep"
 
@@ -46,6 +61,10 @@ class OracleEngine:
         self.plen = np.zeros(self.n_envs, dtype=np.int64)
         self.ret = np.zeros(self.n_envs)
         self.ended = np.zeros(self.n_envs, dtype=bool)      # MwEnvState.ended
+        self.start = [None] * self.n_envs                   # each env's episode start, in the form of a snaps entry
+        self.log = [[] for _ in range(self.n_envs)]         # what changed each env since its episode start
+        self.saved = {}                                     # save_states rows, by records buffer
+        self.rows = {}                                      # goal rows, by rows buffer
 
     def set_options(self, max_steps, tos, seed):
         self.max_steps, self.tos = int(max_steps), bool(tos)
@@ -57,8 +76,10 @@ class OracleEngine:
     def set_goal_sets(self, first, count):
         raise NotImplementedError("the device sampler has no CPU stand-in")
 
-    def _start(self, e, sid):
-        slot, rv, po, rv1 = self.snaps[sid]
+    def _start(self, e, sid, start=None):
+        """Restarts env e from `start` (default: snapshot `sid`) and records `sid` as its snapshot id."""
+        start = self.snaps[sid] if start is None else start
+        slot, rv, po, rv1 = start
         assert slot == self.env_model[e]
         env = self.envs[e]
         lo, _ = env.random_reset_space()
@@ -70,6 +91,7 @@ class OracleEngine:
         if rv1 is not None:
             del env._get_state_rand_vec
         self.snap[e], self.plen[e], self.ret[e], self.ended[e] = sid, 0, 0.0, False
+        self.start[e], self.log[e] = start, []
         return o
 
     def reset(self, snapshot_ids, obs, env_ids=None):
@@ -81,6 +103,24 @@ class OracleEngine:
         for e in np.nonzero(mask.numpy())[0]:
             obs[e, :39] = torch.from_numpy(self._start(e, int(snapshot_ids[e])).astype(np.float32))
 
+    def build_goal_rows(self, mask, rand_vec, rand_vec_pass1, partial, rows):
+        defs = self.rows.setdefault(rows.data_ptr(), {})
+        f = rows.view(torch.float32)
+        for e in np.nonzero(mask.numpy())[0]:
+            rv = rand_vec[e].numpy().copy()
+            rv1 = rv if rand_vec_pass1 is None else rand_vec_pass1[e].numpy().copy()
+            defs[e] = (int(self.env_model[e]), rv, bool(partial[e]), rv1)
+            ok = np.isfinite(rv).all() and np.isfinite(rv1).all()
+            f[e, _OBS:_OBS + 39] = 0.0 if ok else float("nan")
+            f[e, _TARGET:_TARGET + 3] = 0.0
+
+    def reset_rows(self, mask, rows, obs):
+        defs = self.rows[rows.data_ptr()]
+        f = rows.view(torch.float32)
+        for e in np.nonzero(mask.numpy())[0]:
+            if torch.isfinite(f[e, _OBS:_OBS + 39]).all():
+                obs[e, :39] = torch.from_numpy(self._start(e, -1, defs[e]).astype(np.float32))
+
     def step(self, actions, obs, reward, term, trunc, info, final_obs, final_info, next_snapshot):
         a = actions.numpy()
         for e, env in enumerate(self.envs):
@@ -91,6 +131,7 @@ class OracleEngine:
                 obs[e, :39] = torch.from_numpy(self._start(e, int(next_snapshot[e])).astype(np.float32))
                 continue
             o, r, _, _, inf = env.step(a[e])
+            self.log[e].append(("step", a[e].copy()))
             self.plen[e] += 1
             self.ret[e] += np.float32(r)
             tr = self.plen[e] >= self.max_steps
@@ -131,12 +172,42 @@ class OracleEngine:
     def set_state(self, st):
         raise NotImplementedError("mid-episode physics restore is tested on the device (tests/test_gpu.py)")
 
+    def save_states(self, records, record_model, hints, mask=None):
+        st = self.get_state()
+        saved = self.saved.setdefault(records.data_ptr(), {})
+        for e in range(self.n_envs) if mask is None else np.nonzero(mask.numpy())[0]:
+            records[e] = torch.from_numpy(np.frombuffer(st[e].tobytes(), dtype=np.uint8).copy())
+            record_model[e] = int(self.env_model[e])
+            saved[e] = (self.start[e], int(self.snap[e]), list(self.log[e]), int(self.plen[e]), float(self.ret[e]),
+                        bool(self.ended[e]))
+
+    def load_states(self, records, record_model, hints, mask=None, src=None):
+        saved = self.saved[records.data_ptr()]
+        for e in range(self.n_envs) if mask is None else np.nonzero(mask.numpy())[0]:
+            s = e if src is None else int(src[e])
+            if not (0 <= s < records.shape[0] and int(record_model[s]) == self.env_model[e]):
+                continue
+            start, sid, log, plen, ret, ended = saved[s]
+            self._start(e, sid, start)
+            env = self.envs[e]
+            for op in log:
+                if op[0] == "step":
+                    env.step(op[1])
+                elif op[0] == "set":
+                    env.data.qpos, env.data.qvel = op[1].copy(), op[2].copy()
+                else:
+                    P.mj_forward(env.model, env.data)
+                    env._get_obs()
+            self.log[e] = list(log)
+            self.plen[e], self.ret[e], self.ended[e] = plen, ret, ended
+
     def set_physics(self, mask, qpos, qvel):
         for e in np.nonzero(mask.numpy())[0]:
             d = self.envs[e].data
             nq, nv = len(d.qpos), len(d.qvel)
             d.qpos = qpos[e, :nq].numpy().copy()
             d.qvel = qvel[e, :nv].numpy().astype(np.float32).astype(np.float64)
+            self.log[e].append(("set", np.array(d.qpos, dtype=np.float64), np.array(d.qvel, dtype=np.float64)))
 
     def get_physics(self, qpos, qvel):
         qpos.zero_(); qvel.zero_()
@@ -150,6 +221,7 @@ class OracleEngine:
             env = self.envs[e]
             P.mj_forward(env.model, env.data)
             obs[e, :39] = torch.from_numpy(env._get_obs().astype(np.float32))
+            self.log[e].append(("observe",))
 
     def query(self, mask, frame=None, pose=None, frames=None, touching=None, main_geom=None):
         for e in np.nonzero(mask.numpy())[0]:

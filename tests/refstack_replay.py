@@ -7,6 +7,9 @@ raised exception, with the arguments the test passed; the log is written to test
 Without it the proxies replay that log: each access must match the recorded one (same path, same arguments, compared
 exactly) and returns the recorded value, so the test compares this package against the reference's outputs as they
 were when the log was written, on any machine.
+
+The fixtures `ref` (the test's session), `gym` and `metaworld` (the proxied modules) are shared by the test modules that
+import them.
 """
 import builtins
 import gzip
@@ -14,6 +17,7 @@ import os
 import pickle
 
 import numpy as np
+import pytest
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 _PLAIN = (type(None), bool, int, float, complex, str, bytes, np.generic, np.dtype)
@@ -160,6 +164,23 @@ class RefSession:
         if isinstance(v, (list, tuple)):
             return type(v)(self._restore(x) for x in v)
         return v
+
+
+@pytest.fixture
+def ref(request):
+    s = RefSession(request.node.name.replace("[", "_").rstrip("]"))
+    yield s
+    s.close()
+
+
+@pytest.fixture
+def gym(ref):
+    return ref.module("gymnasium")
+
+
+@pytest.fixture
+def metaworld(ref, gym):
+    return ref.module("metaworld")
 
 
 class _Proxy:

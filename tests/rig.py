@@ -1,6 +1,7 @@
-"""What the GPU tests that compare against the golden trajectories share (tests/test_gpu.py and its neighbours,
-scripts/gpu_diag.py): the fixtures, the tolerance, the known float32-vs-float64 sensitivities, and `Rig`, N envs of one
-task on the raw engine."""
+"""What the GPU tests (tests/test_gpu*.py) and scripts/gpu_diag.py share: the `torch_cuda` fixture, random actions and
+the DISABLED restarts of the vector env (`acts`, `reset_ended`), its steady-state MT50 setup (`steady_mt50`), the golden
+trajectories, the tolerance, the known float32-vs-float64 sensitivities, and `Rig`, N envs of one task on the raw
+engine.  A test module takes the fixture with `from rig import torch_cuda`."""
 import glob
 import os
 
@@ -9,6 +10,37 @@ import pytest
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 TOL = 1e-4
+
+
+@pytest.fixture(scope="module")
+def torch_cuda():
+    import torch
+    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
+    return torch
+
+
+def acts(torch, rng, n, dev):
+    return torch.from_numpy(rng.uniform(-1, 1, size=(n, 4)).astype(np.float32)).to(dev)
+
+
+def reset_ended(env, out):
+    """DISABLED autoreset: restart the envs whose episode ended in this step; returns the reset observation (or None)."""
+    if env.autoreset_mode != "Disabled":
+        return None
+    return env.reset_torch(env.torch.logical_or(out[2], out[3]).bool()).clone()
+
+
+def steady_mt50(torch, mode="SameStep", n=4096, seed=42):
+    """MT50 with one-hot ids in `mode`, episode phases spread over 0..499 by bench.py's `stagger`, 20 steps in."""
+    import bench
+    from metaworld_b200.vector_env import make_mt_envs
+    env = make_mt_envs("MT50", seed=seed, num_envs=n, use_one_hot=True, autoreset_mode=mode)
+    env.reset_torch()
+    bench.stagger(env, seed)
+    rng = np.random.default_rng(seed + 1)
+    for _ in range(20):
+        reset_ended(env, env.step_torch(acts(torch, rng, n, env.device)))
+    return env
 
 
 def _tasks_with_goldens():

@@ -1,14 +1,14 @@
 """CPU suite: saved env states (`MetaWorldVecEnv.save_states` / `load_states`).  The C entry points' argument checks in
-both libraries, and the REAL host code of the vector env on the float64 oracle stand-in (tests/oracle_branch.py, whose
+both libraries, and the REAL host code of the vector env on the float64 oracle stand-in (tests/oracle_engine.py, whose
 save_states / load_states replay a saved row's episode on the target env): the host mirrors, the optional wrappers' rows
-and the returned observations follow `src`, and a restored env replays the original run exactly.  The device side is
-tests/test_gpu_branch.py."""
+and the returned observations follow `src`, and a restored env replays the original run exactly, also from a state
+saved on a goal row.  The device side is tests/test_gpu_branch.py."""
 import os
 
 import numpy as np
 import pytest
 
-from oracle_branch import branch_vec_env as _ours
+from oracle_engine import oracle_vec_env as _ours
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -86,6 +86,32 @@ def test_load_restores_ended_marks_mirrors_wrapper_rows_and_replays():
     for t, (a, b) in enumerate(zip(orig, got)):
         assert _same(a, b), t
     assert v.get_attr("curr_path_length") == orig_len
+
+
+def test_state_saved_on_a_goal_row_replays():
+    """MT10 x 2 replicas on the oracle: every other env restarts at a new goal (`reset_goals`) and is saved two steps
+    later, while it runs on its goal row.  Loading the save back with `src` = identity restores the running goals and
+    replays the following steps exactly, through the episode ends in the window."""
+    N = 20
+    v = _ours("mt", "MT10", seed=3, num_goals=2, num_envs=N, max_episode_steps=6)
+    v.reset()
+    acts = np.random.default_rng(1).uniform(-1, 1, size=(9, N, 4)).astype(np.float32)
+    _run(v, acts[:1])
+    mask = np.arange(N) % 2 == 0
+    rv, rv1 = v.sample_goals(np.random.default_rng(0), mask)
+    v.reset_goals(rv, mask, rv1)
+    _run(v, acts[1:3])
+    v.call("toggle_sample_tasks_on_reset", False)         # a restart then draws the same task in both runs
+    st = v.save_states()
+    assert np.all(v.engine.get_state()["snapshot"][mask] == -1)
+    goals = v.get_attr("_last_rand_vec")
+    orig = _run(v, acts[3:])
+    assert any(x[3].any() for x in orig)                  # the window holds episode ends
+    v.load_states(st, src=np.arange(N))
+    assert all(np.array_equal(x, y) for x, y in zip(v.get_attr("_last_rand_vec"), goals))
+    got = _run(v, acts[3:])
+    for t, (a, b) in enumerate(zip(orig, got)):
+        assert _same(a, b), t
 
 
 def test_load_checks_its_inputs_before_changing_anything():

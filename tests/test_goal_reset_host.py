@@ -1,6 +1,6 @@
 """CPU suite: episodes at new goals (unfrozen rand_vec).  The C entry points' argument checks in both libraries; the bare
 env's `_freeze_rand_vec = False` / `seeded_rand_vec` resets against the reference's own class; and the REAL host code of
-`MetaWorldVecEnv.reset_goals` on the float64 oracle stand-in (tests/oracle_goals.py).  The reference side is replayed
+`MetaWorldVecEnv.reset_goals` on the float64 oracle stand-in (tests/oracle_engine.py).  The reference side is replayed
 from tests/golden/refstack_<test>.pkl.gz (tests/refstack_replay.py); with METAWORLD_REFERENCE=<Meta-World checkout> it
 runs live and rewrites those files.  The device side is tests/test_gpu_goal_reset.py."""
 import os
@@ -9,8 +9,8 @@ import numpy as np
 import pytest
 import torch
 
-from oracle_goals import GoalOracleEngine, goal_vec_env
-from refstack_replay import RefSession
+from oracle_engine import OracleEngine, oracle_vec_env
+from refstack_replay import gym, metaworld, ref  # noqa: F401
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -28,19 +28,6 @@ def test_goal_entry_points_reject_a_null_engine(built):
             assert lib.mw_last_error().decode() == f"{name}: mw_set_envs not called", (so, name, args)
 
 
-@pytest.fixture
-def ref(request):
-    s = RefSession(request.node.name.replace("[", "_").rstrip("]"))
-    yield s
-    s.close()
-
-
-@pytest.fixture
-def metaworld(ref):
-    ref.module("gymnasium")
-    return ref.module("metaworld")
-
-
 # reach / pick-place / sweep-into: rejection loops (sweep-into's against its constant goal); drawer-close: reset_model
 # moves a static body, and the reset observation shows where the first pass put it
 @pytest.mark.parametrize("mode", ["global", "seeded"])
@@ -56,7 +43,7 @@ def test_bare_env_unfrozen_resets_match_reference_class(metaworld, name, mode):
     rb = metaworld.MT1(name, seed=3)
     ob = B.MT1(name, seed=3, n_goals=3)
     renv = rb.train_classes[name]()
-    oenv = SawyerXYZEnvB200(name, engine=GoalOracleEngine([name]))
+    oenv = SawyerXYZEnvB200(name, engine=OracleEngine([name]))
     renv.set_task(rb.train_tasks[0]); oenv.set_task(ob.train_tasks[0])
     renv._freeze_rand_vec = False; oenv._freeze_rand_vec = False
     if mode == "seeded":
@@ -102,7 +89,7 @@ def test_reset_goals_checks_inputs_and_equals_a_masked_reset_from_snapshots():
     it, holds the same pending draws and RNG states) and the next masked reset draws what `w`'s does."""
     N = 20
     kw = dict(seed=5, num_goals=3, num_envs=N, max_episode_steps=9, normalize_observations=True)
-    v, u, w = (goal_vec_env("mt", "MT10", **kw) for _ in range(3))
+    v, u, w = (oracle_vec_env("mt", "MT10", **kw) for _ in range(3))
     rng = np.random.default_rng(1)
     acts = rng.uniform(-1, 1, size=(8, N, 4)).astype(np.float32)
     mask = np.arange(N) % 2 == 0

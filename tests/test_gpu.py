@@ -13,15 +13,9 @@ import pytest
 from builds import run_digests, variant_lib
 from rig import (GOLD, POLICY_FAILS_ON_REFERENCE_GLUE, SENSITIVE_CONTACT_RICH, SENSITIVE_ONE_STEP, SENSITIVE_OPEN_LOOP,
                  SENSITIVE_RESET, TOL, Rig, _TOUCH, _params, _report, _tasks_with_goldens)
+from rig import torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch
 
 
 @pytest.mark.parametrize("task", _params(SENSITIVE_RESET))

@@ -3,14 +3,9 @@ produce are bitwise the episodes of the default SAME_STEP run: only where each t
 import numpy as np
 import pytest
 
+from rig import torch_cuda  # noqa: F401
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch
 
 
 def _actions(ep, k):

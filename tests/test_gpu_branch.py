@@ -4,39 +4,10 @@ mismatch is refused, and neither call synchronises with the host."""
 import numpy as np
 import pytest
 
+from rig import acts, reset_ended, steady_mt50
+from rig import torch_cuda  # noqa: F401
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch
-
-
-def _acts(torch, rng, n, dev):
-    return torch.from_numpy(rng.uniform(-1, 1, size=(n, 4)).astype(np.float32)).to(dev)
-
-
-def _reset_ended(env, out):
-    """DISABLED autoreset: restart the envs whose episode ended in this step; returns the reset observation (or None)."""
-    if env.autoreset_mode != "Disabled":
-        return None
-    return env.reset_torch(env.torch.logical_or(out[2], out[3]).bool()).clone()
-
-
-def _steady_mt50(torch, mode, n=4096, seed=42):
-    """MT50 with one-hot ids in `mode`, episode phases spread over 0..499 as in bench.py, 20 steps in."""
-    from metaworld_b200.vector_env import make_mt_envs
-    env = make_mt_envs("MT50", seed=seed, num_envs=n, use_one_hot=True, autoreset_mode=mode)
-    env.reset_torch()
-    st = env.engine.get_state()
-    st["path_len"] = ((np.arange(n) * 500 // n)[np.random.default_rng(seed).permutation(n)]).astype(np.float32)
-    env.engine.set_state(st)
-    rng = np.random.default_rng(seed + 1)
-    for _ in range(20):
-        _reset_ended(env, env.step_torch(_acts(torch, rng, n, env.device)))
-    return env
 
 
 @pytest.mark.parametrize("mode", ["SameStep", "NextStep", "Disabled"])
@@ -44,15 +15,15 @@ def test_restore_replays_bitwise(torch_cuda, mode):
     """MT50 @ 4096 in steady state: save, 60 steps with autoresets (DISABLED: the ended envs reset with reset_torch(mask)),
     restore, the same 60 steps again: every output tensor and the final state records are bitwise equal."""
     torch = torch_cuda
-    env = _steady_mt50(torch, mode)
+    env = steady_mt50(torch, mode)
     rng = np.random.default_rng(5)
-    A = [_acts(torch, rng, env.num_envs, env.device) for _ in range(60)]
+    A = [acts(torch, rng, env.num_envs, env.device) for _ in range(60)]
 
     def run():
         outs = []
         for a in A:
             out = [x.clone() for x in env.step_torch(a)]
-            outs.append(out + [_reset_ended(env, out)])
+            outs.append(out + [reset_ended(env, out)])
         return outs, env.engine.get_state()
 
     states = env.save_states()
@@ -81,7 +52,7 @@ def test_forks_equal_their_source(torch_cuda):
     env.reset_torch()
     rng = np.random.default_rng(3)
     for _ in range(k):
-        env.step_torch(_acts(torch, rng, n, dev))
+        env.step_torch(acts(torch, rng, n, dev))
     src = torch.arange(n, device=dev) % 10                          # env e has task e % 10; its first env is e % 10
     qpos = env.engine.get_state()["qpos"]
     assert not np.array_equal(qpos[10], qpos[0])
@@ -89,7 +60,7 @@ def test_forks_equal_their_source(torch_cuda):
     assert torch.equal(obs, obs[src])
     ended_at = None
     for t in range(k, M + 2):
-        out = env.step_torch(_acts(torch, rng, 10, dev)[src].contiguous())
+        out = env.step_torch(acts(torch, rng, 10, dev)[src].contiguous())
         end = bool(out[3][0])
         for x in (env.d_final_obs,) + tuple(out[1:]) if end else out:
             assert torch.equal(x, x[src]), t
@@ -148,7 +119,7 @@ def test_optional_wrappers_restore_bitwise(torch_cuda):
                        reward_normalization_method="gymnasium", recurrent_info_in_obs=True)
     env.reset_torch()
     rng = np.random.default_rng(1)
-    A = [_acts(torch, rng, n, env.device) for _ in range(40)]
+    A = [acts(torch, rng, n, env.device) for _ in range(40)]
     for a in A[:10]:
         env.step_torch(a)
     states = env.save_states()
@@ -176,10 +147,10 @@ def test_model_mismatch_is_refused(torch_cuda):
     dev = env.device
     env.reset_torch()
     rng = np.random.default_rng(4)
-    env.step_torch(_acts(torch, rng, n, dev))
+    env.step_torch(acts(torch, rng, n, dev))
     states = env.save_states()
     for _ in range(3):
-        env.step_torch(_acts(torch, rng, n, dev))
+        env.step_torch(acts(torch, rng, n, dev))
     before = env.engine.get_state()
     src = np.arange(n)
     src[[3, 50]] = [4, 61]                                          # another task
@@ -212,7 +183,7 @@ def test_save_and_load_do_not_synchronise(torch_cuda):
     dev = env.device
     env.reset_torch()
     rng = np.random.default_rng(0)
-    A = [_acts(torch, rng, n, dev) for _ in range(6)]
+    A = [acts(torch, rng, n, dev) for _ in range(6)]
     src = torch.roll(torch.arange(n, device=dev), 10)
     mask = torch.arange(n, device=dev) % 2 == 0
     for a in A:

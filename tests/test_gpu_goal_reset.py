@@ -5,40 +5,10 @@ goals; the bare env's unfrozen resets equal its frozen path for the same vectors
 import numpy as np
 import pytest
 
+from rig import acts, reset_ended, steady_mt50
+from rig import torch_cuda  # noqa: F401
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch
-
-
-def _acts(torch, rng, n, dev):
-    return torch.from_numpy(rng.uniform(-1, 1, size=(n, 4)).astype(np.float32)).to(dev)
-
-
-def _steady_mt50(torch, mode, n=4096, seed=42):
-    """MT50 with one-hot ids in `mode`, episode phases spread over 0..499 as in bench.py, 20 steps in (the setup of
-    tests/test_gpu_branch.py)."""
-    from metaworld_b200.vector_env import make_mt_envs
-    env = make_mt_envs("MT50", seed=seed, num_envs=n, use_one_hot=True, autoreset_mode=mode)
-    env.reset_torch()
-    st = env.engine.get_state()
-    st["path_len"] = ((np.arange(n) * 500 // n)[np.random.default_rng(seed).permutation(n)]).astype(np.float32)
-    env.engine.set_state(st)
-    rng = np.random.default_rng(seed + 1)
-    for _ in range(20):
-        _reset_ended(env, env.step_torch(_acts(torch, rng, n, env.device)))
-    return env
-
-
-def _reset_ended(env, out):
-    """DISABLED autoreset: restart the envs whose episode ended in this step; returns the reset observation (or None)."""
-    if env.autoreset_mode != "Disabled":
-        return None
-    return env.reset_torch(env.torch.logical_or(out[2], out[3]).bool()).clone()
 
 
 def _without_snapshot(rec):
@@ -106,7 +76,7 @@ def test_reset_goals_torch_equals_a_masked_reset_from_snapshots(torch_cuda, mode
     the snapshot field of the rows still on their goal (-1); the unmasked envs' records, hints and observation rows are
     untouched, and the snapshot table does not grow."""
     torch = torch_cuda
-    a, b = _steady_mt50(torch, mode), _steady_mt50(torch, mode)
+    a, b = steady_mt50(torch, mode), steady_mt50(torch, mode)
     N, dev = a.num_envs, a.device
     mask_np = np.arange(N) % 2 == 0
     rows = np.nonzero(mask_np)[0]
@@ -133,11 +103,11 @@ def test_reset_goals_torch_equals_a_masked_reset_from_snapshots(torch_cuda, mode
     assert all(np.array_equal(got[e], rv[e, :len(got[e])]) for e in rows[:64])
     rng = np.random.default_rng(5)
     for t in range(200):
-        act = _acts(torch, rng, N, dev)
+        act = acts(torch, rng, N, dev)
         oa, ob = a.step_torch(act), b.step_torch(act)
         for x, y in zip(oa, ob):
             assert torch.equal(x, y), (mode, t)
-        ra, rb = _reset_ended(a, oa), _reset_ended(b, ob)
+        ra, rb = reset_ended(a, oa), reset_ended(b, ob)
         assert (ra is None and rb is None) or torch.equal(ra, rb), (mode, t)
     sa, sb = a.engine.get_state(), b.engine.get_state()
     still = sa["snapshot"] == -1
@@ -156,11 +126,11 @@ def test_reset_goals_does_not_synchronise(torch_cuda):
     env.reset_torch()
     dev = env.device
     rng = np.random.default_rng(2)
-    env.step_torch(_acts(torch, rng, 200, dev))
+    env.step_torch(acts(torch, rng, 200, dev))
     rv, rv1 = (torch.from_numpy(x).to(dev) for x in env.sample_goals(np.random.default_rng(3)))
     mask = torch.from_numpy(np.arange(200) % 3 == 0).to(dev)
     env.reset_goals_torch(rv, mask, rv1)                 # first use: allocates the buffers, builds the float64 env table
-    act = _acts(torch, rng, 200, dev)
+    act = acts(torch, rng, 200, dev)
     torch.cuda.synchronize()
     torch.cuda.set_sync_debug_mode("error")
     try:
@@ -192,7 +162,7 @@ def test_fresh_goal_loop(torch_cuda):
     env.reset_goals_torch(P[0], None, P1[0])
     count += 1
     rng = np.random.default_rng(4)
-    A = [_acts(torch, rng, N, dev) for _ in range(600)]
+    A = [acts(torch, rng, N, dev) for _ in range(600)]
     torch.cuda.synchronize()
     torch.cuda.set_sync_debug_mode("error")
     try:
@@ -225,7 +195,7 @@ def test_goal_state_survives_save_load_and_checkpoint(torch_cuda):
     dev = env.device
     env.reset_torch()
     rng = np.random.default_rng(6)
-    A = [_acts(torch, rng, N, dev) for _ in range(70)]
+    A = [acts(torch, rng, N, dev) for _ in range(70)]
     for a in A[:5]:
         env.step_torch(a)
     rv, rv1 = env.sample_goals(np.random.default_rng(1), np.arange(N) % 2 == 1)

@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 
 from rig import POLICY_FAILS_ON_REFERENCE_GLUE, _report
+from rig import torch_cuda  # noqa: F401
 from test_policies import ALL_SOURCES, build_shim, expert_rows, host_actions
 
 pytestmark = pytest.mark.gpu
@@ -22,13 +23,6 @@ N_GOALS, MAX_STEPS = 50, 500
 # soccer goals (seed 42) on the oracle; the device scored 0.76 there.  At 500 steps (the acceptance test) it reaches 0.80 on
 # both.
 BELOW_BAR_AT_300_STEPS = {"soccer-v3": "soccer's policy solves 36/50 of MT50's goals within 300 steps on the float64 oracle too"}
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch
 
 
 @pytest.fixture(scope="module")

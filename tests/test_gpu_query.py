@@ -5,20 +5,13 @@ import os
 import numpy as np
 import pytest
 
-from rig import GOLD, Rig, _tasks_with_goldens
-from test_gpu_set_state import _steady_mt50
+from rig import GOLD, Rig, _tasks_with_goldens, steady_mt50
+from rig import torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 _HLO = np.array([-0.525, 0.348, -0.0525], dtype=np.float32)     # SawyerXYZEnv._HAND_SPACE
 _HHI = np.array([0.525, 1.025, 0.7], dtype=np.float32)
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch
 
 
 def _actions(torch, env, steps, seed=7):
@@ -29,7 +22,7 @@ def test_frame_is_bitwise_the_step_observation(torch_cuda):
     """MT50 @ 4096 in steady state, 30 steps with autoresets: after every step the queried frame equals the step's
     obs[:, :18], bitwise on the unclipped columns 3..17 and after the hand-space clip on columns 0..2."""
     torch = torch_cuda
-    env = _steady_mt50(torch)
+    env = steady_mt50(torch)
     A = _actions(torch, env, 30)
     lo, hi = torch.from_numpy(_HLO).to(env.device), torch.from_numpy(_HHI).to(env.device)
     for t in range(30):
@@ -48,7 +41,7 @@ def test_query_has_no_side_effects(torch_cuda):
     """The same 30 steps with and without a full query (16 named frames and touching) between them: bitwise equal step
     outputs and final device records, and no fault bit."""
     torch = torch_cuda
-    env = _steady_mt50(torch)
+    env = steady_mt50(torch)
     st0 = env.engine.get_state()
     A = _actions(torch, env, 30)
     bodies = ("hand", "rightpad", "leftpad", "obj", "rightclaw", "leftclaw")

@@ -5,39 +5,17 @@ import os
 import numpy as np
 import pytest
 
-from rig import GOLD, SENSITIVE_OPEN_LOOP, TOL, Rig, _params
+from rig import GOLD, SENSITIVE_OPEN_LOOP, TOL, Rig, _params, steady_mt50
+from rig import torch_cuda  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch
-
-
-def _steady_mt50(torch, n=4096, seed=42):
-    """MT50 with one-hot ids, episode phases spread over 0..499 as in bench.py, 20 steps in."""
-    from metaworld_b200.vector_env import make_mt_envs
-    env = make_mt_envs("MT50", seed=seed, num_envs=n, use_one_hot=True)
-    env.reset()
-    st = env.engine.get_state()
-    p = (np.arange(n) * 500 // n)[np.random.default_rng(seed).permutation(n)]
-    st["path_len"] = p.astype(np.float32)
-    env.engine.set_state(st)
-    env._ep_len[:] = p
-    rng = np.random.default_rng(seed + 1)
-    for _ in range(20):
-        env.step_torch(torch.from_numpy(rng.uniform(-1, 1, size=(n, 4)).astype(np.float32)).to(env.device))
-    return env
 
 
 def test_setting_every_env_to_its_own_state_changes_nothing(torch_cuda):
     """MT50 @ 4096 in steady state: set_state_torch(*get_state_torch()) on all envs, then 50 steps (autoresets included):
     every step's outputs and the final device records are bitwise those of the same run without the call."""
     torch = torch_cuda
-    env = _steady_mt50(torch)
+    env = steady_mt50(torch)
     st0 = env.engine.get_state()
     A = torch.from_numpy(np.random.default_rng(7).uniform(-1, 1, size=(50, env.num_envs, 4)).astype(np.float32)).to(env.device)
 

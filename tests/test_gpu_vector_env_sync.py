@@ -3,16 +3,11 @@ autoreset mode, with and without the optional wrappers."""
 import numpy as np
 import pytest
 
+from rig import torch_cuda  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 
 WRAPPERS = dict(normalize_observations=True, reward_normalization_method="gymnasium", recurrent_info_in_obs=True)
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch
 
 
 @pytest.mark.parametrize("wrappers", [False, True])

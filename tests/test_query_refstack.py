@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 from oracle_engine import OracleEngine
-from refstack_replay import RefSession
+from refstack_replay import RefSession, gym, metaworld  # noqa: F401
 
 ATOL = 2e-6
 _HLO, _HHI = np.array([-0.525, 0.348, -0.0525]), np.array([0.525, 1.025, 0.7])
@@ -32,12 +32,6 @@ def ref(request):
     s = _SnapshotSession(request.node.name.replace("[", "_").rstrip("]"))
     yield s
     s.close()
-
-
-@pytest.fixture
-def metaworld(ref):
-    ref.module("gymnasium")
-    return ref.module("metaworld")
 
 
 def _outcome(fn):

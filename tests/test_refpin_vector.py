@@ -9,26 +9,9 @@ import numpy as np
 import pytest
 
 from oracle_engine import oracle_vec_env as _ours
-from refstack_replay import RefSession
+from refstack_replay import gym, metaworld, ref  # noqa: F401
 
 KEYS = ("success", "near_object", "grasp_success", "grasp_reward", "in_place_reward", "obj_to_target", "unscaled_reward")
-
-
-@pytest.fixture
-def ref(request):
-    s = RefSession(request.node.name.replace("[", "_").rstrip("]"))
-    yield s
-    s.close()
-
-
-@pytest.fixture
-def gym(ref):
-    return ref.module("gymnasium")
-
-
-@pytest.fixture
-def metaworld(ref, gym):
-    return ref.module("metaworld")
 
 
 def _compare_rollout(ref, ours, steps, seed, atol=2e-6):

@@ -1,30 +1,22 @@
 """CPU suite: the vector env's numpy calls and their `_torch` twins share one last observation and one set of ended marks.
 An env that replaces every other call of a fixed sequence with its torch twin returns what an all-numpy twin returns, in
-every autoreset mode, with and without the optional wrappers.  Runs the REAL host code on the float64 oracle stand-in,
-with the saved-state stand-in of tests/oracle_branch.py and the goal-row stand-in of tests/oracle_goals.py combined.
-The pseudorandom task selection never re-draws a task on reset, so no device sampler is needed."""
+every autoreset mode, with and without the optional wrappers.  Runs the REAL host code on the float64 oracle stand-in
+(tests/oracle_engine.py).  The pseudorandom task selection never re-draws a task on reset, so no device sampler is
+needed."""
 import numpy as np
 import pytest
 import torch
 
-from oracle_branch import BranchOracleEngine
-from oracle_goals import GoalOracleEngine
+from oracle_engine import oracle_vec_env
 
 N = 20                                  # MT10 x 2 replicas
 WRAPPERS = dict(normalize_observations=True, reward_normalization_method="gymnasium", recurrent_info_in_obs=True)
 
 
-class _Engine(BranchOracleEngine, GoalOracleEngine):
-    """Saved states and goal rows.  A state saved while its env runs on a goal row (snapshot id -1) cannot be replayed
-    by the saved-state stand-in, so the sequence below saves only before its goal reset."""
-
-
 def _env(mode, wrappers):
-    from metaworld_b200 import benchmarks as B
-    from metaworld_b200.vector_env import make_mt_envs
     kw = WRAPPERS if wrappers else {}
-    return make_mt_envs("MT10", engine=_Engine(list(B.MT10)), seed=4, num_goals=3, num_envs=N, max_episode_steps=4,
-                        task_select="pseudorandom", autoreset_mode=mode, **kw)
+    return oracle_vec_env("mt", "MT10", seed=4, num_goals=3, num_envs=N, max_episode_steps=4, task_select="pseudorandom",
+                          autoreset_mode=mode, **kw)
 
 
 def _host(x):
