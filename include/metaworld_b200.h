@@ -86,6 +86,27 @@ int mw_step(mw_engine*, const float* actions, float* obs, int obs_stride, float*
             unsigned char* terminated, unsigned char* truncated, float* info, int info_stride, float* final_obs,
             float* final_info, const int* next_snapshot, void* stream);
 
+/* Open-loop rollouts of k candidate action sequences from every env's current state, leaving the envs untouched (no
+ * reference counterpart; the closest pattern is copy.deepcopy of a SawyerXYZEnv, then step() per candidate).  Row (c, i)
+ * starts from env i's state record, the one the next mw_step starts from, and its step h takes actions[c, h, i].  Each
+ * step is mw_step's step bit for bit: the action clip, the mocap and gripper command, 5 substeps and the sixth pass,
+ * the live target, the clipped frame-stacked observation, the reward of the raw action, TimeLimit truncation at
+ * max_episode_steps (counted from the record's path length) and terminate_on_success.  The step that ends a row's episode
+ * reports its flags and terminal observation; every later step of that row has flag 4 and zero reward, info and obs.
+ * There is no autoreset: no snapshot or device-sampler draw, no change of the episode counter.  A row whose env is
+ * marked ended (NEXT_STEP / DISABLED, before its restart) is ended from step 0.  Nothing of the engine changes: not the
+ * state records, the separating-axis hints, the fault bits (mw_get_faults), diagnostics, launch-order keys or profile;
+ * only mw_get_counters [0] counts the launch.  A row's own fault bits 1 / 2 / 4 / 8, OR-ed over its live steps, and its
+ * dropped contacts go to diag.  The launch runs the env CTA table k times, in the last mw_step's order.  Asynchronous on
+ * `stream`; neither allocates nor synchronises.  MW_ERR_ARG for a NULL required buffer, k < 1 or horizon < 1;
+ * MW_ERR_STATE for a NULL engine or one without mw_set_envs.  All arrays DEV:
+ *   actions [k, horizon, n_envs, 4] f32; reward [k, horizon, n_envs] f32; info [k, horizon, n_envs, 7] f32 (mw_step's
+ *   info columns 0..6); flags [k, horizon, n_envs] u8: 1 terminated, 2 truncated, 4 ended before this step; obs
+ *   [k, horizon, n_envs, 39] f32 or NULL; diag [k, n_envs, 2] i32: fault bits, contacts dropped; hints [k * n_envs,
+ *   MW_NCONV (128), 4] f32: caller-owned workspace, row c * n_envs + i starts as env i's separating-axis hints.         */
+int mw_rollout(mw_engine*, int k, int horizon, const float* actions, float* reward, float* info, unsigned char* flags,
+               float* obs, int* diag, float* hints, void* stream);
+
 /* gymnasium.vector.AutoresetMode of mw_step; other values fail with MW_ERR_ARG.  Takes effect at the next launch. */
 enum mw_autoreset_mode { MW_AUTORESET_SAME_STEP = 0, MW_AUTORESET_NEXT_STEP = 1, MW_AUTORESET_DISABLED = 2 };
 int mw_set_autoreset_mode(mw_engine*, int mode);

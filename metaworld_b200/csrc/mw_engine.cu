@@ -45,7 +45,7 @@ struct EngineDev {
   unsigned long long* model_cycles;                  // [n_models][2]: warp cycles, env steps (drives mw_rebalance)
   unsigned* env_cost;                                // [n_envs] solver work of each env's previous step (orders the envs of a model, k_order_envs)
   unsigned* env_cycles;                              // [n_envs] cycles each env's warp spent in its previous k_step = duration of its CTA (orders the CTAs, k_order_blocks)
-  float4* sep_hint;                                  // [n_envs][MW_NCONV] separating-axis hints of the general convex pairs (k_step only; mw_collide)
+  float4* sep_hint;                                  // [n_envs][MW_NCONV] separating-axis hints of the general convex pairs (k_step; k_rollout reads it and runs on a copy; mw_collide)
   unsigned* env_prof;                                // optional [n_envs][16] per-env phase cycles / event counts of the last step (mw_set_profiling)
   int n_envs, max_steps, terminate_on_success; unsigned long long seed;
   int autoreset_mode;                                // MW_AUTORESET_* (mw_set_autoreset_mode)
@@ -95,7 +95,7 @@ DEV void stage_model(BlockShared* bs, const unsigned char* src, unsigned bytes, 
 }
 
 // wires a warp into its CTA's convex-pair queue (mw_physics.cuh: CtaShare); visible to the other warps after the first PHASE_SYNC
-// `sep`: the env's row of the separating-axis hint table (k_step); the other kernels run without hints
+// `sep`: the env's row of the separating-axis hint table (k_step; k_rollout: its workspace row); the other kernels run without hints
 DEV void join_cta(BlockShared* bs, WarpShared* wsa, WarpScratch* w, int warp, int live_warps, float4* sep = nullptr) {
   if (threadIdx.x == 0) { bs->cs.q_head = 0; bs->cs.nwarp = live_warps; bs->cs.peer_stride = (int)sizeof(WarpShared); bs->cs.peer0 = (unsigned char*)wsa; }
   if ((threadIdx.x & 31) == 0) { w->cta = &bs->cs; w->warp_in_cta = warp; w->ncand = 0; w->prof_on = 0; w->nblk1 = mw_tree_split((const MwModel*)bs->model); w->sep = sep; }
@@ -110,9 +110,8 @@ __device__ void eng_sim(const TaskCtx& c, int nstep, int lane) {
 }
 
 // ---------------------------------------------------------------- state <-> scratch
-DEV void load_env(WarpShared* ws, const MwEnvState* src, int lane) {
-  ((float4*)&ws->es)[lane] = ((const float4*)src)[lane];     // 32 lanes x 16 B = the whole 512 B record
-  SYNCW();
+// the scratch state of the record in ws->es (k_rollout: between two steps, which store and load the record in shared memory)
+DEV void scratch_from_record(WarpShared* ws, int lane) {
   WarpScratch* w = &ws->w;
   if (lane < MW_MAXNQ) { w->qposd[lane] = ws->es.qpos[lane]; w->qpos[lane] = (real)w->qposd[lane]; }
   if (lane < MW_MAXDOF) { w->qvel[lane] = ws->es.qvel[lane]; w->warm[lane] = ws->es.warm[lane]; }
@@ -120,12 +119,20 @@ DEV void load_env(WarpShared* ws, const MwEnvState* src, int lane) {
   if (lane == 0) { w->mocap_quat[0] = 1; w->mocap_quat[1] = 0; w->mocap_quat[2] = 1; w->mocap_quat[3] = 0; w->ctrl[0] = w->ctrl[1] = 0; }
   SYNCW();
 }
-DEV void store_env(WarpShared* ws, MwEnvState* dst, int lane) {
+DEV void record_from_scratch(WarpShared* ws, int lane) {
   WarpScratch* w = &ws->w;
   if (lane < MW_MAXNQ) ws->es.qpos[lane] = w->qposd[lane];
   if (lane < MW_MAXDOF) { ws->es.qvel[lane] = (float)w->qvel[lane]; ws->es.warm[lane] = (float)w->warm[lane]; }
   if (lane < 3) { ws->es.mocap_pos[lane] = (float)w->mocap_pos[lane]; ws->es.shift[lane] = (float)w->shift[lane]; }
   SYNCW();
+}
+DEV void load_env(WarpShared* ws, const MwEnvState* src, int lane) {
+  ((float4*)&ws->es)[lane] = ((const float4*)src)[lane];     // 32 lanes x 16 B = the whole 512 B record
+  SYNCW();
+  scratch_from_record(ws, lane);
+}
+DEV void store_env(WarpShared* ws, MwEnvState* dst, int lane) {
+  record_from_scratch(ws, lane);
   ((float4*)dst)[lane] = ((const float4*)&ws->es)[lane];
 }
 
@@ -142,7 +149,7 @@ struct CtaWarp {
 
 // Entry of every CTA kernel for work item `blk` of `bt`: stages the item's model, then places each warp on its env, wires
 // its global scratch slots and joins it to the CTA's convex-pair queue (`hints`: with the env's row of the separating-axis
-// hint table; k_step only).  Barriers: every thread of the CTA takes part in the two __syncthreads of stage_model; a warp
+// hint table e.sep_hint; k_step, and k_rollout with its workspace there).  Barriers: every thread of the CTA takes part in the two __syncthreads of stage_model; a warp
 // past count[blk] then returns false and its kernel returns before join_cta, so the CTA's phase barriers count only the
 // count[blk] warps that have an env.
 DEV bool cta_enter(const EngineDev& e, const BlockTable& bt, int blk, CtaWarp& cw, bool hints = false) {
@@ -217,32 +224,28 @@ DEV int sample_snapshot(const EngineDev& e, int env, float episode) {
 }
 
 // ---------------------------------------------------------------- kernels
-// DEFERRED = false: SAME_STEP autoreset; true: NEXT_STEP or DISABLED (e.autoreset_mode tells which).  Two instantiations,
-// so that the default path carries none of the code of the other modes (the kernel is bound by instruction fetch)
-template <bool DEFERRED>
-__global__ void __launch_bounds__(BLOCK_THREADS, 1)
-k_step(EngineDev e, const int* __restrict__ block_order, BlockTable bt, const float* __restrict__ actions, float* __restrict__ obs_out, int obs_stride,
-       float* __restrict__ reward, unsigned char* __restrict__ terminated, unsigned char* __restrict__ truncated,
-       float* __restrict__ info_out, int info_stride, float* __restrict__ final_obs, float* __restrict__ final_info, const int* __restrict__ next_snapshot,
-       const int* __restrict__ block_live) {
-  const int blk = block_order[blockIdx.x];             // launch slot -> CTA work item (costliest first, see k_order_*)
-  if (block_live && !block_live[blk]) return;          // the other decomposition of this model's head is running (k_order_blocks)
-  CtaWarp cw;
-  if (!cta_enter(e, bt, blk, cw, /*hints=*/true)) return;
+// One env step of the warp's env from its loaded record (SawyerXYZEnv.step, sawyer_xyz_env.py:580-642, with TimeLimit and
+// AutoTerminateOnSuccessWrapper, wrappers.py:207-230): the action clip, the mocap and gripper command, 5 substeps and the
+// sixth pass, path length, task_live_update, the clipped observation (frame stack committed) into ws->obs, the reward of
+// the raw action, the infos into ws->info[0..6] and done into ws->info[7].  `action`: the env's 4 floats.  Every warp of
+// the CTA runs it (phase barriers).  k_step and k_rollout share it, so that a rollout step is a step bit for bit.  Lane 0
+// fills the reward and the flags and then runs `tail(out)`, the caller's use of them, in the same branch.
+struct StepOut {
+  real rew; bool term, trunc;
+  int iters, dropped, ncon_max, nefc_max, solver_work, cand_total;   // summed / largest over the 6 passes
+  long long t_phys;                                                  // MW_CLK at the end of the physics
+};
+template <class Lane0Tail>
+DEV StepOut env_step(const EngineDev& e, const CtaWarp& cw, const float* __restrict__ action, Lane0Tail&& tail) {
   BlockShared* bs = cw.bs; WarpShared* ws = cw.ws; WarpScratch* w = cw.w; const MwModel* m = cw.m;
-  const int mi = cw.mi, lane = cw.lane, env = cw.env;
-  enter_env(e, cw, e.prof != nullptr);
-  // NEXT_STEP / DISABLED: an env whose episode ended in the previous call still runs its physics below, so that its warp
-  // takes part in the CTA's phase barriers, and the result is discarded in the tail (restart, or nothing at all)
-  const bool ended = DEFERRED && ws->es.ended != 0.f;
-  const long long t_begin = MW_CLK(w);
-  const long long t_cta = e.env_cycles ? mw_clock() : 0ll;
+  const int lane = cw.lane;
+  StepOut o;
   real act[4];
-  for (int i = 0; i < 4; i++) act[i] = fmin(fmax((real)actions[4 * env + i], (real)-1), (real)1);
+  for (int i = 0; i < 4; i++) act[i] = fmin(fmax((real)action[i], (real)-1), (real)1);
   TaskCtx c = task_ctx(e, cw, act);
   // set_xyz_action (sawyer_xyz_env.py:320-336) + ctrl = [a3, -a3] (:595)
   if (lane < 3) w->mocap_pos[lane] = fmin(fmax(w->mocap_pos[lane] + act[lane] * (real)0.01, (real)bs->tc.mocap_lo[lane]), (real)bs->tc.mocap_hi[lane]);
-  if (lane == 0) { w->ctrl[0] = (real)actions[4 * env + 3]; w->ctrl[1] = -(real)actions[4 * env + 3]; }
+  if (lane == 0) { w->ctrl[0] = (real)action[3]; w->ctrl[1] = -(real)action[3]; }
   SYNCW();
   int iters = 0, dropped = 0, ncon_max = 0, nefc_max = 0, solver_work = 0, cand_total = 0;
   for (int s = 0; s < 5; s++) {
@@ -257,50 +260,78 @@ k_step(EngineDev e, const int* __restrict__ block_order, BlockTable bt, const fl
     iters += w->solver_iter; dropped += w->ncon_dropped; ncon_max = max(ncon_max, w->ncon); nefc_max = max(nefc_max, w->nefc);
     solver_work += (w->solver_iter + 1) * (w->nefc + 4 * w->ncon + 24); cand_total += w->ncand;
   } else mw_forward_kinematics_only(m, w, lane);
-  bool done = false;
-  const long long t_phys = MW_CLK(w);
+  o.iters = iters; o.dropped = dropped; o.ncon_max = ncon_max; o.nefc_max = nefc_max; o.solver_work = solver_work; o.cand_total = cand_total;
+  o.t_phys = MW_CLK(w);
   if (lane == 0) {
     ws->es.path_len += 1.f;
     task_live_update(c);
     make_obs(c, ws->obs);
     real obsr[39]; for (int i = 0; i < 39; i++) obsr[i] = ws->obs[i];
     real rew, inf[INFO_N];
-    real raw_act[4]; for (int i = 0; i < 4; i++) raw_act[i] = actions[4 * env + i];
+    real raw_act[4]; for (int i = 0; i < 4; i++) raw_act[i] = action[i];
     c.action = raw_act;
     task_reward(c, obsr, &rew, inf);
     for (int i = 0; i < INFO_N; i++) ws->info[i] = (float)inf[i];
     ws->es.ep_return += (float)rew;
-    bool trunc = ws->es.path_len >= (float)e.max_steps;
-    bool term = e.terminate_on_success && inf[INFO_SUCCESS] == (real)1;
-    ws->info[7] = (term || trunc) ? 1.f : 0.f;
+    o.trunc = ws->es.path_len >= (float)e.max_steps;
+    o.term = e.terminate_on_success && inf[INFO_SUCCESS] == (real)1;
+    ws->info[7] = (o.term || o.trunc) ? 1.f : 0.f;
+    o.rew = rew;
+    tail(o);
+  }
+  return o;
+}
+
+// DEFERRED = false: SAME_STEP autoreset; true: NEXT_STEP or DISABLED (e.autoreset_mode tells which).  Two instantiations,
+// so that the default path carries none of the code of the other modes (the kernel is bound by instruction fetch)
+template <bool DEFERRED>
+__global__ void __launch_bounds__(BLOCK_THREADS, 1)
+k_step(EngineDev e, const int* __restrict__ block_order, BlockTable bt, const float* __restrict__ actions, float* __restrict__ obs_out, int obs_stride,
+       float* __restrict__ reward, unsigned char* __restrict__ terminated, unsigned char* __restrict__ truncated,
+       float* __restrict__ info_out, int info_stride, float* __restrict__ final_obs, float* __restrict__ final_info, const int* __restrict__ next_snapshot,
+       const int* __restrict__ block_live) {
+  const int blk = block_order[blockIdx.x];             // launch slot -> CTA work item (costliest first, see k_order_*)
+  if (block_live && !block_live[blk]) return;          // the other decomposition of this model's head is running (k_order_blocks)
+  CtaWarp cw;
+  if (!cta_enter(e, bt, blk, cw, /*hints=*/true)) return;
+  WarpShared* ws = cw.ws; WarpScratch* w = cw.w;
+  const int mi = cw.mi, lane = cw.lane, env = cw.env;
+  enter_env(e, cw, e.prof != nullptr);
+  // NEXT_STEP / DISABLED: an env whose episode ended in the previous call still runs its physics below, so that its warp
+  // takes part in the CTA's phase barriers, and the result is discarded in the tail (restart, or nothing at all)
+  const bool ended = DEFERRED && ws->es.ended != 0.f;
+  const long long t_begin = MW_CLK(w);
+  const long long t_cta = e.env_cycles ? mw_clock() : 0ll;
+  bool done = false;
+  const StepOut s = env_step(e, cw, actions + 4 * env, [&](const StepOut& s) {
     if (!ended) {
-      reward[env] = (float)rew; terminated[env] = term; truncated[env] = trunc;
-      if (info_stride >= 9) { info_out[(size_t)env * info_stride + 7] = (float)rew; info_out[(size_t)env * info_stride + 8] = (float)((int)term + 2 * (int)trunc); }   // packed record: one D2H copy
-      { bool fin = isfinite((float)rew); for (int i = 0; i < 39; i++) fin = fin && isfinite(ws->obs[i]); if (!fin) w->fault |= MW_FAULT_NONFINITE; }
-      e.diag[3 * env] += dropped; e.diag[3 * env + 1] += iters; e.diag[3 * env + 2] |= w->fault;
+      reward[env] = (float)s.rew; terminated[env] = s.term; truncated[env] = s.trunc;
+      if (info_stride >= 9) { info_out[(size_t)env * info_stride + 7] = (float)s.rew; info_out[(size_t)env * info_stride + 8] = (float)((int)s.term + 2 * (int)s.trunc); }   // packed record: one D2H copy
+      { bool fin = isfinite((float)s.rew); for (int i = 0; i < 39; i++) fin = fin && isfinite(ws->obs[i]); if (!fin) w->fault |= MW_FAULT_NONFINITE; }
+      e.diag[3 * env] += s.dropped; e.diag[3 * env + 1] += s.iters; e.diag[3 * env + 2] |= w->fault;
     } else if (e.autoreset_mode == MW_AUTORESET_DISABLED) e.diag[3 * env + 2] |= MW_FAULT_STEP_AFTER_END;   // the discarded pass reports nothing else
-    w->prof[7] = MW_CLK(w) - t_phys; w->prof[8] = MW_CLK(w) - t_begin;
+    w->prof[7] = MW_CLK(w) - s.t_phys; w->prof[8] = MW_CLK(w) - t_begin;
     // launch-order key: the cycles this env spent in its constraint solver + constraint assembly.  The whole-step time
     // is the same for all warps of a CTA (they wait for each other at every phase boundary) and would keep light envs
     // glued to the heavy one they were once grouped with; the collision phase is shared across the CTA (CtaShare); the
     // other phases cost the same for every env of a model.  What is left to group by is the solver.
     const long long own = w->prof[8] - w->prof[12];
     // (a work estimate from counters rather than the cycle clock: Newton iterations weighted by the rows they touch)
-    e.env_cost[env] = (unsigned)solver_work;
+    e.env_cost[env] = (unsigned)s.solver_work;
     if (e.env_cycles) { long long d = mw_clock() - t_cta; e.env_cycles[env] = (unsigned)(d > 0xFFFFFFFFll ? 0xFFFFFFFFll : d); }
     w->prof[6] = own - w->prof[7] - (w->prof[0] + w->prof[1] + w->prof[3] + w->prof[4] + w->prof[5]);   // euler + glue
-  }
+  });
   SYNCW();
   if (e.prof) {     // profiling runs only (mw_set_profiling): summed phase counters, per-model cost, per-env record
     if (lane < 16) atomicAdd(e.prof + lane, (unsigned long long)w->prof[lane]);
     if (lane == 0 && e.model_cycles) { atomicAdd(e.model_cycles + 2 * mi, (unsigned long long)w->prof[8]); atomicAdd(e.model_cycles + 2 * mi + 1, 1ull); }
     if (e.env_prof) {
       if (lane < 13) e.env_prof[MW_ENVPROF_W * env + lane] = (unsigned)(w->prof[lane] > 0xFFFFFFFFll ? 0xFFFFFFFFll : w->prof[lane]);
-      if (lane == 13) e.env_prof[MW_ENVPROF_W * env + 13] = (unsigned)iters;
-      if (lane == 14) e.env_prof[MW_ENVPROF_W * env + 14] = (unsigned)ncon_max;
-      if (lane == 15) e.env_prof[MW_ENVPROF_W * env + 15] = (unsigned)nefc_max;
+      if (lane == 13) e.env_prof[MW_ENVPROF_W * env + 13] = (unsigned)s.iters;
+      if (lane == 14) e.env_prof[MW_ENVPROF_W * env + 14] = (unsigned)s.ncon_max;
+      if (lane == 15) e.env_prof[MW_ENVPROF_W * env + 15] = (unsigned)s.nefc_max;
       if (lane == 16) e.env_prof[MW_ENVPROF_W * env + 16] = (unsigned)blockIdx.x;
-      if (lane == 17) e.env_prof[MW_ENVPROF_W * env + 17] = (unsigned)cand_total;      // convex candidate pairs this env queued
+      if (lane == 17) e.env_prof[MW_ENVPROF_W * env + 17] = (unsigned)s.cand_total;      // convex candidate pairs this env queued
       if (lane == 18 || lane == 19) e.env_prof[MW_ENVPROF_W * env + lane] = (unsigned)w->prof[lane - 5];   // hint tests / rejections by this warp
     }
   }
@@ -346,6 +377,55 @@ k_step(EngineDev e, const int* __restrict__ block_order, BlockTable bt, const fl
     ((float4*)(e.state + env))[lane] = ((const float4*)&ws->es)[lane];
     for (int i = lane; i < 39; i += 32) obs_out[(size_t)env * obs_stride + i] = sp->obs[i];
   }
+}
+
+// Open-loop rollouts (mw_rollout) over the CTA table replicated K times: launch slot s runs work item block_order[s / K]
+// (the last step's order) for candidate k = s % K.  Each warp loads its env's record once and runs H env_steps with the
+// actions actions[k, h, env]; between two steps the record goes through shared memory as store_env / load_env would
+// take it through HBM, and it is never stored.  The env's live hint row is copied into workspace row k * n_envs + env,
+// which the row's collision passes read and update instead, so the live hint table is never written.  Every warp runs
+// every step, so that the CTA's warps meet at each phase barrier; a row whose episode has ended (an ended record of
+// NEXT_STEP / DISABLED, or an earlier step of the rollout) discards its result, as DEFERRED k_step does, and reports
+// flag 4 with zero outputs.  Outputs of step h go to row (k * H + h) * n_envs + env; diag[k, env] = the OR of the live
+// steps' fault bits, their dropped contacts.  Nothing of the engine is written: not the records, hints, diag, the
+// launch-order keys or the profile.
+__global__ void __launch_bounds__(BLOCK_THREADS, 1)
+k_rollout(EngineDev e, const int* __restrict__ block_order, BlockTable bt, const int* __restrict__ block_live, int K, int H,
+          const float* __restrict__ actions, float* __restrict__ reward, float* __restrict__ info, unsigned char* __restrict__ flags,
+          float* __restrict__ obs, int* __restrict__ diag, float4* __restrict__ hints) {
+  const int blk = block_order[blockIdx.x / K], k = blockIdx.x % K;
+  if (block_live && !block_live[blk]) return;          // the other decomposition of this model's head (k_order_blocks)
+  const int N = e.n_envs;
+  EngineDev er = e;
+  er.sep_hint = hints + (size_t)k * N * MW_NCONV;      // cta_enter wires workspace row k * N + env
+  CtaWarp cw;
+  if (!cta_enter(er, bt, blk, cw, /*hints=*/true)) return;
+  WarpShared* ws = cw.ws; WarpScratch* w = cw.w;
+  const int lane = cw.lane, env = cw.env;
+  for (int i = lane; i < MW_NCONV; i += 32) er.sep_hint[(size_t)env * MW_NCONV + i] = e.sep_hint[(size_t)env * MW_NCONV + i];
+  enter_env(e, cw, 0);                                 // its SYNCW also orders the hint copy before the first pass
+  bool ended = e.autoreset_mode != MW_AUTORESET_SAME_STEP && ws->es.ended != 0.f;
+  int fault = 0, dropped = 0;
+  for (int h = 0; h < H; h++) {
+    const size_t row = ((size_t)k * H + h) * N + env;
+    env_step(e, cw, actions + 4 * row, [&](const StepOut& s) {
+      if (!ended) {
+        bool fin = isfinite((float)s.rew); for (int i = 0; i < 39; i++) fin = fin && isfinite(ws->obs[i]);
+        if (!fin) w->fault |= MW_FAULT_NONFINITE;
+        fault |= w->fault; dropped += s.dropped;
+      }
+      reward[row] = ended ? 0.f : (float)s.rew;
+      flags[row] = ended ? 4 : (unsigned char)((int)s.term + 2 * (int)s.trunc);
+      w->fault = 0;
+    });
+    SYNCW();
+    if (lane < INFO_N) info[row * INFO_N + lane] = ended ? 0.f : ws->info[lane];
+    if (obs) for (int i = lane; i < 39; i += 32) obs[row * 39 + i] = ended ? 0.f : ws->obs[i];
+    ended = ended || ws->info[7] != 0.f;
+    record_from_scratch(ws, lane);
+    scratch_from_record(ws, lane);
+  }
+  if (lane == 0) { const size_t r = (size_t)k * N + env; diag[2 * r] = fault; diag[2 * r + 1] = dropped; }
 }
 
 // The reference's reset() (reset_model, mj_resetData, reset_model) of the warp's model with rand_vec rv1 in the first
@@ -1051,6 +1131,7 @@ int mw_create(mw_engine** out, int device, int n_models, const void* models, con
   CK(cudaFuncSetAttribute(k_order_blocks, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(unsigned long long) * MW_SORT_MAX)));
   CK(cudaFuncSetAttribute(k_step<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_step<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
+  CK(cudaFuncSetAttribute(k_rollout, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_snapshot, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_goal_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
   CK(cudaFuncSetAttribute(k_substeps, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes()));
@@ -1200,6 +1281,20 @@ int mw_step(mw_engine* E, const float* actions, float* obs, int obs_stride, floa
   if (launched(E, 3)) return MW_ERR_CUDA;
   E->env_steps += (unsigned long long)E->n_envs;
   return MW_OK;
+}
+
+int mw_rollout(mw_engine* E, int k, int horizon, const float* actions, float* reward, float* info, unsigned char* flags,
+               float* obs, int* diag, float* hints, void* stream) {
+  if (!actions || !reward || !info || !flags || !diag || !hints || k < 1 || horizon < 1) return fail(MW_ERR_ARG, "mw_rollout: bad arguments");
+  if (!E || !E->d_state.p) return fail(MW_ERR_STATE, "mw_rollout: mw_set_envs not called");
+  CK(cudaSetDevice(E->device));
+  const EnvBlocks& B = E->blk;
+  const int nb = B.n_split ? B.n_blocks_total : B.n_blocks;
+  if ((long long)k * nb > 0x7fffffffll) return fail(MW_ERR_ARG, "mw_rollout: bad arguments");
+  if (ensure_epa(E, (size_t)k * nb)) return MW_ERR_CUDA;   // launch slots address the scratch unless it is by SM
+  k_rollout<<<k * nb, BLOCK_THREADS, smem_bytes(), (cudaStream_t)stream>>>(E->dev(), B.order.p, E->blocks(), B.n_split ? B.live.p : nullptr,
+      k, horizon, actions, reward, info, flags, obs, diag, (float4*)hints);
+  return launched(E, 1);
 }
 
 int mw_evaluate(mw_engine* E, const float* actions, const float* obs, int obs_stride, float* out, void* stream) {

@@ -56,6 +56,7 @@ def _load(path):
     L.mw_get_snapshots.argtypes = [vp, ip, ip, vp]
     L.mw_reset.argtypes = [vp, ip, vp, vp, vp, ip, vp]
     L.mw_step.argtypes = [vp, vp, vp, ip, vp, vp, vp, vp, ip, vp, vp, vp, vp]
+    L.mw_rollout.argtypes = [vp, ip, ip, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mw_set_autoreset_mode.argtypes = [vp, ip]
     L.mw_reset_masked.argtypes = [vp, vp, vp, vp, ip, vp]
     L.mw_build_goal_rows.argtypes = [vp, vp, vp, vp, vp, vp, vp]
@@ -307,6 +308,16 @@ class Engine:
         _ck(lib().mw_step(self.h, self._p(actions), self._p(obs), obs.stride(0), self._p(reward), self._p(terminated),
                           self._p(truncated), self._p(info), info.stride(0), self._p(final_obs), self._p(final_info),
                           self._p(next_snapshot), self._stream()))
+
+    def rollout(self, actions, reward, info, flags, obs, diag, hints):
+        """Open-loop rollouts from every env's current state, leaving the envs untouched (mw_rollout): `actions` float32
+        [K, H, n_envs, 4]; outputs `reward` float32 [K, H, n_envs], `info` float32 [K, H, n_envs, 7], `flags` uint8
+        [K, H, n_envs] (1 terminated, 2 truncated, 4 ended before this step), `obs` float32 [K, H, n_envs, 39] or None,
+        `diag` int32 [K, n_envs, 2] (fault bits, contacts dropped); `hints` float32 [K * n_envs, NCONV, 4] is workspace.
+        Contiguous device tensors; asynchronous on the current stream."""
+        K, H = actions.shape[0], actions.shape[1]
+        _ck(lib().mw_rollout(self.h, K, H, self._p(actions), self._p(reward), self._p(info), self._p(flags), self._p(obs),
+                             self._p(diag), self._p(hints), self._stream()))
 
     AUTORESET_MODES = {"SameStep": 0, "NextStep": 1, "Disabled": 2}     # gymnasium.vector.AutoresetMode values -> MW_AUTORESET_*
 

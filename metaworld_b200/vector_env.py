@@ -24,6 +24,7 @@ draw the reference would make at that point or rewound, so the task sequence and
 from __future__ import annotations
 
 import base64
+from typing import Any, NamedTuple
 
 import numpy as np
 
@@ -177,6 +178,25 @@ class EnvStates:
         return self.records.view(torch.float32)[:, _ENDED_WORD] != 0
 
 
+class Rollout(NamedTuple):
+    """What `MetaWorldVecEnv.rollout_torch` returns for K candidate action sequences of H steps over N envs: device tensors
+    (numpy arrays from `rollout`).  Row [k, h, e] is step h of candidate k from env e's current state.
+    * `reward` float32 [K, H, N], `info` float32 [K, H, N, 7] (INFO_KEYS order): the base env's raw reward and infos;
+    * `terminated`, `truncated` bool [K, H, N]: the step that ends the row's episode;
+    * `ended` bool [K, H, N]: the episode ended before this step (reward, info and obs are zero);
+    * `obs` float32 [K, H, N, 39] or None: the base observation, the terminal one on the ending step;
+    * `faults` int32 [K, N]: fault bits 1 / 2 / 4 / 8 (`Engine.FAULTS`) OR-ed over the row's live steps;
+    * `contacts_dropped` int32 [K, N]: the contacts the row's live steps dropped."""
+    reward: Any
+    info: Any
+    terminated: Any
+    truncated: Any
+    ended: Any
+    obs: Any
+    faults: Any
+    contacts_dropped: Any
+
+
 class MetaWorldVecEnv(_gym.VectorEnvBase):
     metadata = {"render_modes": [], "autoreset_mode": "same_step"}
 
@@ -270,6 +290,7 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
         # input of `expert_actions_torch`
         self._d_raw = self.d_obs
         self._d_expert_ids = None
+        self._rollout_hints = None                     # rollout_torch's hint workspace [K * N, NCONV, 4], grown with K
         self.d_final_obs39 = torch.zeros(N, 39, device=dev)
         self.d_reward = torch.zeros(N, device=dev)
         self.d_term = torch.zeros(N, dtype=torch.uint8, device=dev)
@@ -1031,6 +1052,56 @@ class MetaWorldVecEnv(_gym.VectorEnvBase):
                 raise ValueError(f"expert_actions needs obs of shape ({self.num_envs}, >= 39), got {o.shape}")
             obs = self.torch.from_numpy(np.ascontiguousarray(o[:, :39], dtype=np.float32)).to(self.device)
         return self.expert_actions_torch(obs).cpu().numpy()
+
+    # ------------------------------------------------------------------ open-loop rollouts (planning)
+    # A rollout answers "from where each env is now, what would each of these K action sequences earn over H steps?"
+    # without moving the envs.  Each step is `step_torch`'s step of the base env, bit for bit, with TimeLimit and
+    # terminate_on_success; a row's episode end is its last live step (no autoreset, no task draw).  The optional
+    # wrappers and one-hot columns are not applied, as in `observe_torch` and `expert_actions_torch`.
+    def rollout_torch(self, actions, obs=False):
+        """Rolls K open-loop action sequences out from every env's current state, H steps each, and leaves every env as it
+        was (state, hints, fault bits, launch order, host mirrors, wrapper statistics).  `actions`: a contiguous float32
+        tensor [K, H, num_envs, 4] on this env's device, K and H >= 1; row (k, e) starts from the state the next
+        `step_torch` of env e would start from and takes `actions[k, h, e]` at its step h.  An env marked ended (NEXT_STEP
+        / DISABLED, before its restart) is ended from step 0.  Returns a `Rollout` of new device tensors (`obs` only when
+        `obs` is true), without host synchronisation; the hint workspace is kept on the env and grown with K."""
+        self._check_started("rollout_torch")
+        t, N = self.torch, self.num_envs
+        if not (isinstance(actions, t.Tensor) and actions.dim() == 4 and actions.shape[0] >= 1 and actions.shape[1] >= 1):
+            raise ValueError(f"actions must be a contiguous float32 tensor of shape (K, H, {N}, 4) with K, H >= 1 on {self.device}")
+        K, H = actions.shape[:2]
+        self._check_tensor("actions", actions, t.float32, (K, H, N, 4), contiguous=True)
+        dev = self.device
+        if self._rollout_hints is None or self._rollout_hints.shape[0] < K * N:
+            self._rollout_hints = t.empty(K * N, NCONV, 4, dtype=t.float32, device=dev)
+        reward = t.empty(K, H, N, device=dev)
+        info = t.empty(K, H, N, 7, device=dev)
+        flags = t.empty(K, H, N, dtype=t.uint8, device=dev)
+        o = t.empty(K, H, N, 39, device=dev) if obs else None
+        diag = t.empty(K, N, 2, dtype=t.int32, device=dev)
+        self.engine.rollout(actions, reward, info, flags, o, diag, self._rollout_hints)
+        return Rollout(reward, info, (flags & 1) != 0, (flags & 2) != 0, (flags & 4) != 0, o, diag[..., 0], diag[..., 1])
+
+    def rollout(self, actions, obs=False):
+        """`rollout_torch` from a numpy float32 array [K, H, num_envs, 4]; returns a `Rollout` of numpy arrays after one
+        synchronisation.  A bad shape or dtype raises ValueError before anything runs; fault bits 1 / 2 / 4 / 8 in any row
+        raise ValueError with `Engine.FAULTS`' message, as `Engine.raise_on_faults` does for `step`."""
+        N = self.num_envs
+        a = np.asarray(actions)
+        if a.dtype != np.float32 or a.ndim != 4 or a.shape[2:] != (N, 4) or a.shape[0] < 1 or a.shape[1] < 1:
+            raise ValueError(f"rollout needs actions as a float32 array of shape (K, H, {N}, 4) with K, H >= 1, got {a.dtype} {a.shape}")
+        self._check_started("rollout")
+        r = self.rollout_torch(self.torch.from_numpy(np.ascontiguousarray(a)).to(self.device), obs)
+        host = [None if x is None else x.to("cpu", non_blocking=True) for x in r]
+        if self.device.type == "cuda":
+            self.torch.cuda.synchronize(self.device)
+        out = Rollout(*(None if x is None else x.numpy() for x in host))
+        bad = np.argwhere(out.faults & 15)
+        if len(bad):
+            k, e = (int(i) for i in bad[0])
+            msgs = [m for b, m in Engine.FAULTS.items() if out.faults[k, e] & b]
+            raise ValueError(f"rollout candidate {k}, env {e}: " + "; ".join(msgs) + f" ({len(bad)} row(s) flagged)")
+        return out
 
     # attribute RPC used by metaworld/evaluation.py:48-169 and the reference tests
     def _current_tasks(self):
